@@ -10,10 +10,11 @@ Workload "1080p-8bit-speed6-me16x16" (one *step* = one pass of the hot path over
     * forward DCT_DCT 16x16 of the winner's residual (forward_transform, forward.rs:71)
       [added once the transform kernels land; reported in config.legs].
   value = candidate blocks evaluated per second, whole job (all ranks).
-  F is sized so that planes + descriptors exceed the 126 MB L2 (config.l2: "inputs>L2").
+  F is sized so that planes + descriptors exceed the 50 MB L2 of an H100 (config.l2: "inputs>L2").
 
 JSON contract: see the task statement; extra objects `roofline`, `cpu_baseline`, `e2e`,
-`clocks`, `gpu_launches`.  `--impl reference` times the CPU oracle (the reference's
+`clocks`, `gpu_launches`.  `--dump-outputs DIR` writes what the last timed step computed as
+DIR/<name>.npy (see step_outputs).  `--impl reference` times the CPU oracle (the reference's
 algorithm restated in C; rav1e itself cannot be built here: no rustc/nasm) with all host
 threads on a bounded sample of the same workload.
 """
@@ -45,7 +46,7 @@ def peaks():
     if os.path.exists(p):
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet 3.35 TB/s)"
 
 
 class ClockSampler:
@@ -183,7 +184,7 @@ def run_reference(args, rank, world):
     }))
 
 
-# ----------------------------------------------------------------------------- B200 arm
+# ----------------------------------------------------------------------------- GPU arm
 def run_b200(args, rank, world, local_rank):
     import torch
     import torch.distributed as dist
@@ -330,6 +331,7 @@ def run_b200(args, rank, world, local_rank):
     l0 = ctx.launches
     ms = timed(step, args.steps)
     launches = ctx.launches - l0
+    outputs = step_outputs(F, nb, n_sad, n_satd, d_sad, d_satd, d_best, d_best2, d_coef) if args.dump_outputs else None
     for _ in range(int(min(2000, max(0, 250.0 / max(ms / args.steps, 1e-3) - args.steps)))):   # ~0.25 s more of the
         step()                                                   # same steps (untimed): clock samples under load
     torch.cuda.synchronize()
@@ -409,13 +411,6 @@ def run_b200(args, rank, world, local_rank):
     alg_bytes = int((n_sad * (BW * BH + 4) + nb * BW * BH) * pairs_per_launch)
     peak, peak_src = peaks()
     achieved = alg_bytes / (ms_sad * 1e-3) / 1e9
-    traffic = None
-    tp = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(tp):
-        with open(tp) as fh:
-            traffic = json.load(fh).get("me_cand_group_u8_16x16_dram_bytes_per_frame_pair")
-            if traffic is not None:
-                traffic = int(traffic * pairs_per_launch)
 
     out = None
     # ---- e2e: same metric through the host-buffer C ABI (H2D + kernels + D2H per frame), on every rank
@@ -429,6 +424,9 @@ def run_b200(args, rank, world, local_rank):
         torch.cuda.set_stream(stream)
     if rank == 0:
         cpu = run_cpu_baseline(blocks)
+        sms = torch.cuda.get_device_properties(local_rank).multi_processor_count
+        mhz = clocks["sm_max_mhz"] or 1980.0        # H100 SXM max SM clock where nvidia-smi is unavailable
+        issue_peak = sms * 4 * mhz * 1e6 / 10
         out = {
             "metric": METRIC, "value": value, "unit": "blocks/s", "n_gpus": world,
             "steps": args.steps, "warmup": max(args.warmup, 3), "ms_per_step": ms / args.steps,
@@ -462,27 +460,74 @@ def run_b200(args, rank, world, local_rank):
                                "algorithmic_GBps": nb * (8 * 23 * 23 * 2 + 256 * 2 + 256 * 4 + 16) / (ms_c4 * 1e-3) / 1e9}}},
             "roofline": {"kernel": "me_cand_group_u8<16,16,SAD> (candidate-list SAD + cost + argmin)",
                          "bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                         "frac": achieved / peak, "traffic": traffic, "peak_source": peak_src,
-                         "traffic_source": "static: ncu dram__bytes of the same 32-pair launch recorded in "
-                                           "profiles/traffic.json (not re-measured in this run)",
+                         "frac": achieved / peak, "traffic": None, "peak_source": peak_src,
                          "algorithmic_bytes_per_launch": alg_bytes,
                          "launch_ms": ms_sad,
-                         # what actually binds this kernel (ncu: DRAM traffic is 0.08x the algorithmic bytes):
-                         # warp-instruction issue.  Floor per candidate in the cooperative loop: 1 LDS.128
-                         # (parameters) + 4 LDS.32 + 2 funnel shifts + 2 VABSDIFF4.ACC + 1 REDUX = 10.
+                         # the other bound of this kernel: warp-instruction issue.  Floor per candidate in the
+                         # cooperative loop: 1 LDS.128 (parameters) + 4 LDS.32 + 2 funnel shifts + 2 VABSDIFF4.ACC
+                         # + 1 REDUX = 10.
                          "issue_roof": {"floor_warp_instr_per_candidate": 10,
-                                        "peak_candidates_per_s": 148 * 4 * 1.965e9 / 10,
+                                        "peak_candidates_per_s": issue_peak,
                                         "achieved_candidates_per_s": n_sad * pairs_per_launch / (ms_sad * 1e-3),
-                                        "frac": n_sad * pairs_per_launch / (ms_sad * 1e-3) / (148 * 4 * 1.965e9 / 10),
-                                        "note": "148 SMs x 4 schedulers x 1 warp instruction per clock at 1965 MHz; "
-                                                "the measured kernel issues ~29 per candidate, issue slots 68 % busy, L1TEX 73 % "
-                                                "(ncu, profiles/prof_r2l_sad_raw.csv, NOTES_r2.md)"}},
+                                        "frac": n_sad * pairs_per_launch / (ms_sad * 1e-3) / issue_peak,
+                                        "note": f"{sms} SMs x 4 schedulers x 1 warp instruction per clock at {mhz:.0f} MHz "
+                                                "(the maximum SM clock nvidia-smi reports)"}},
             "cpu_baseline": cpu, "e2e": e2e, "clocks": clocks, "gpu_launches": int(launches),
         }
         if tiles4k is not None:
             out["strong_scaling_4k_tiles"] = tiles4k
+        if outputs is not None:
+            dump_outputs(args.dump_outputs, outputs)
         print(json.dumps(out))
     finish(world, dist)
+
+
+DUMP_LIMIT = 64 << 20           # bytes --dump-outputs may write
+# Rows kept of each output: all of them when there are fewer, else a fixed seeded sample.  At the caps the files
+# hold 2 MB of block indices + 10.5 MB of winners + 2 x 12 MB of candidate values and indices + 16.9 MB of
+# coefficients and their block indices = 54.6 MB, whatever --frames is.
+DUMP_BLOCKS = 1 << 18           # blocks whose SAD and SATD winners are kept (the default 32 frames have 261,120)
+DUMP_CANDIDATES = 1 << 20       # per-candidate SADs, and per-candidate SATDs, kept
+DUMP_COEF_BLOCKS = 16384        # blocks whose 256 coefficients are kept
+
+
+def _sample(seed, n, k):
+    """Sorted indices of min(n, k) of n rows: all of them when n <= k, else a sample fixed by `seed`."""
+    return np.arange(n) if n <= k else np.sort(np.random.default_rng(seed).choice(n, k, replace=False))
+
+
+def step_outputs(F, nb, n_sad, n_satd, d_sad, d_satd, d_best, d_best2, d_coef):
+    """What one step hands its caller, copied to the host: the SAD and SATD winners of the blocks, the SAD and the
+    SATD of the candidates, and the winners' coefficients, each whole or as a seeded sample (DUMP_*), with the
+    indices of the rows kept.  u64 costs and indices go to float64, everything else fits float32 exactly."""
+    import torch
+    from rav1e_b200 import backend as B
+    pick = lambda t, i: t[torch.from_numpy(i).to(t.device)].cpu().numpy()
+    out = {}
+    blk = _sample(1, F * nb, DUMP_BLOCKS)
+    out["block_index"] = blk.astype(np.float64)
+    for name, d in (("sad_winner", d_best), ("satd_winner", d_best2)):
+        r = pick(d.view(F * nb, 16), blk).reshape(-1).view(B.ME_RESULT_DTYPE)
+        out[name + "_cost"] = r["cost"].astype(np.float64)
+        for k in ("sad", "mv_row", "mv_col"):
+            out[f"{name}_{k}"] = r[k].astype(np.float32)
+    for seed, name, d, n in ((2, "sad_candidates", d_sad, F * n_sad), (3, "satd_candidates", d_satd, F * n_satd)):
+        idx = _sample(seed, n, DUMP_CANDIDATES)
+        out[name] = pick(d.view(torch.int32), idx).view(np.uint32).astype(np.float32)
+        out[name + "_index"] = idx.astype(np.float64)
+    cb = _sample(4, F * nb, DUMP_COEF_BLOCKS)
+    out["coef"] = pick(d_coef.view(F * nb, BW * BH), cb).astype(np.float32)
+    out["coef_block_index"] = cb.astype(np.float64)
+    total = sum(a.nbytes for a in out.values())
+    if total > DUMP_LIMIT:
+        raise RuntimeError(f"--dump-outputs: {total} bytes exceed the {DUMP_LIMIT}-byte limit")
+    return out
+
+
+def dump_outputs(dirname, outputs):
+    os.makedirs(dirname, exist_ok=True)
+    for name, a in outputs.items():
+        np.save(os.path.join(dirname, name + ".npy"), a)
 
 
 def finish(world, dist):
@@ -503,7 +548,7 @@ def finish(world, dist):
     os._exit(0)
 
 
-# ----------------------------------------------------------------------------- B200 arm, 4K tiles
+# ----------------------------------------------------------------------------- GPU arm, 4K tiles
 W4K, H4K = 3840, 2160
 TILE_COLS_LOG2, TILE_ROWS_LOG2 = 2, 1     # 4 x 2 tiles of 15 x 17 superblocks (BASELINE configs[4])
 
@@ -1097,7 +1142,11 @@ def main():
     ap.add_argument("--graph", action="store_true", help="4k-tiles at N > 1: capture the step (incl. the NCCL all-gather) in a CUDA graph")
     ap.add_argument("--pairs-per-launch", type=int, default=32,
                     help="frame pairs served by one launch of each leg (b200_*_multi_dev); 1 = a launch per pair")
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="write what the last timed 1080p step computed as DIR/<name>.npy (float32 / float64, <= 64 MB)")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl != "b200" or args.workload == "4k-tiles"):
+        ap.error("--dump-outputs dumps the 1080p GPU workload (--impl b200, --workload auto or 1080p)")
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))

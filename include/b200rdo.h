@@ -1,5 +1,5 @@
 /*
- * b200rdo.h — C ABI of the B200-native backend for rav1e's RDO inner loop.
+ * b200rdo.h — C ABI of the H100-native (sm_90a) backend for rav1e's RDO inner loop.
  *
  * Drop-in boundary: rav1e selects a kernel backend per file with a `cfg_if!` module swap
  * (src/dist.rs:10-18, src/mc.rs:10-18, src/predict.rs:16-24, src/cdef.rs:20-28,
@@ -39,7 +39,7 @@ typedef enum {
   B200_OK = 0,
   B200_ERR_CUDA = 1,  /* a CUDA runtime call failed */
   B200_ERR_ARG = 2,   /* precondition violated (the reference would assert!/panic) */
-  B200_ERR_NODEV = 3, /* no usable sm_100 device */
+  B200_ERR_NODEV = 3, /* no usable CUDA device */
   B200_ERR_OOM = 4
 } b200_status;
 
@@ -173,7 +173,7 @@ int b200_me_candidates_dev(b200_ctx *ctx, const b200_plane *cur, const b200_plan
 
 /* The same over `npairs` (cur, ref) plane pairs in ONE launch — the reference evaluates every
  * allowed reference frame of every superblock in turn (estimate_tile_motion, me.rs:178-212) and
- * runs tiles and frames concurrently; a 30 us launch per pair leaves a B200 mostly ramping up and
+ * runs tiles and frames concurrently; a launch per pair leaves the GPU mostly ramping up and
  * draining, so the pairs share a grid.  Blocks, candidates, offsets, pmv and the outputs are the
  * concatenation pair after pair: pair k owns blocks [pair_block_end[k-1], pair_block_end[k]) and
  * candidates [pair_cand_end[k-1], pair_cand_end[k]) (HOST arrays, npairs entries; the last entries

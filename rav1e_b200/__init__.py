@@ -1,4 +1,4 @@
-"""rav1e_b200 — B200-native (sm_100a) backend for rav1e's RDO inner loop.
+"""rav1e_b200 — CUDA backend (sm_90a, H100) for rav1e's RDO inner loop.
 
 The product is the C-ABI shared library `libb200rdo.so` (include/b200rdo.h) built from
 rav1e_b200/csrc/*.cu.  This Python package is plumbing for tests, bench.py and

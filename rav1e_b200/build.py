@@ -1,4 +1,4 @@
-"""In-tree build of the CUDA backend -> rav1e_b200/libb200rdo.so (sm_100a only).
+"""In-tree build of the CUDA backend -> rav1e_b200/libb200rdo.so (sm_90a only).
 
 nvcc cross-compiles without a GPU.  Objects go to build/ (git-ignored); the .so stays in
 the package directory so it travels to the GPU box with the gpurun snapshot.
@@ -16,7 +16,7 @@ OBJ = os.path.join(ROOT, "build", "obj")
 LIB = os.path.join(PKG, "libb200rdo.so")
 NVCC = os.environ.get("NVCC") or shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
 HOSTCXX = "/usr/bin/g++"
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC,-Wall,-Wno-unused-function,-Wno-unknown-pragmas",
          "-ccbin", HOSTCXX, "--expt-relaxed-constexpr"]
 

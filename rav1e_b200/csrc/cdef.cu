@@ -1,5 +1,5 @@
 // cdef.cu — CDEF direction search and constrained directional filter (rav1e src/cdef.rs) for
-// sm_100a, batched over every 8x8 block of a frame plane.
+// sm_90a, batched over every 8x8 block of a frame plane.
 //
 //   cdef_find_dir_kernel   one thread per 8x8 luma block: the 8 directional partial-sum costs
 //                          (cdef.rs:84-143) held in registers, first-max direction, variance.

@@ -14,7 +14,7 @@
 
 #include "../../include/b200rdo.h"
 
-#define B200_NUM_SMS 148
+#define B200_NUM_SMS 132  /* H100 SXM; replaced by the device's count at context creation */
 
 struct b200_ctx {
   int device = 0;
@@ -133,8 +133,8 @@ __device__ __forceinline__ unsigned long long b200_mv_cost(uint32_t sad, int mv_
                                                            int p0_row, int p0_col, int p1_row,
                                                            int p1_col, uint32_t lambda,
                                                            int allow_hp) {
-  // (skipping the second rate when the predictors are equal was measured slower: a branch in every
-  // candidate's cost, profiles/NOTES_r2.md)
+  // (no skipping of the second rate when the predictors are equal: that puts a branch in every
+  // candidate's cost)
   const uint32_t r1 = b200_mv_rate(mv_row, mv_col, p0_row, p0_col, allow_hp);
   const uint32_t r2 = b200_mv_rate(mv_row, mv_col, p1_row, p1_col, allow_hp) + 1;
   const uint32_t rate = r1 < r2 ? r1 : r2;

@@ -1,4 +1,4 @@
-// fwd_txfm.cu — batched 2-D forward transforms (rav1e src/transform/forward.rs:71-161) for sm_100a.
+// fwd_txfm.cu — batched 2-D forward transforms (rav1e src/transform/forward.rs:71-161) for sm_90a.
 //
 // One thread owns one whole column (pass 1) and then one whole row (pass 2) of a block in
 // registers and runs the straight-line lifting network on it (txfm_networks.cuh); the

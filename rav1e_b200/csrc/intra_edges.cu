@@ -1,4 +1,4 @@
-// intra_edges.cu — get_intra_edges for batches of transform blocks (sm_100a).
+// intra_edges.cu — get_intra_edges for batches of transform blocks (sm_90a).
 //
 //   get_intra_edges                     src/partition.rs:639-898
 //   has_top_right / has_bottom_left     src/recon_intra.rs:174-255, :374-452

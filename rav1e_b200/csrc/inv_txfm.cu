@@ -1,4 +1,4 @@
-// inv_txfm.cu — inverse transform + reconstruction for batches of transform blocks (sm_100a).
+// inv_txfm.cu — inverse transform + reconstruction for batches of transform blocks (sm_90a).
 //
 //   rust::inverse_transform_add   src/transform/inverse.rs:1637-1704
 //   INV_TXFM_FNS                  :1593-1623   INV_INTERMEDIATE_SHIFTS :1710-1711

@@ -1,4 +1,4 @@
-// ipred.cu — batched AV1 intra prediction (rav1e src/predict.rs:705-1505) for sm_100a.
+// ipred.cu — batched AV1 intra prediction (rav1e src/predict.rs:705-1505) for sm_90a.
 //
 // One CTA per (block, mode) item: the RDO loop evaluates ~13 modes per block from the same
 // neighbour pixels (rdo.rs:1470-1505), so a launch carries blocks x modes items that all read a

@@ -1,4 +1,4 @@
-// lookahead.cu — the frame-wide, dependence-free consumers of the SATD / intra kernels (sm_100a).
+// lookahead.cu — the frame-wide, dependence-free consumers of the SATD / intra kernels (sm_90a).
 //
 //   Plane::downsampled + Plane::pad        v_frame 0.3.9 (off disk); src/encoder.rs:476-477 builds the half
 //                                          and quarter resolution planes of the ME pyramid with it

@@ -1,4 +1,4 @@
-// mc.cu — batched 8-tap sub-pel motion compensation (rav1e src/mc.rs:250-479) for sm_100a.
+// mc.cu — batched 8-tap sub-pel motion compensation (rav1e src/mc.rs:250-479) for sm_90a.
 //
 // One warp per predicted block (up to 8 blocks per CTA).  The (w+7) x (h+7) source footprint is
 // staged once in shared memory; the separable filter then runs as the reference's four cases (copy / V only /

@@ -1,4 +1,4 @@
-// me_kernels.cu — batched motion-estimation distortion for sm_100a.
+// me_kernels.cu — batched motion-estimation distortion for sm_90a.
 //
 // Replaces, for thousands of candidates per launch, the serial loop
 //   get_fullpel_mv_rd -> compute_mv_rd -> get_sad / get_satd     (rav1e src/me.rs:1386-1461,
@@ -31,8 +31,7 @@
 #define B200_SAD_THREADS 256  // CTA size of the SAD instantiations of the grouped kernel
 #endif
 #ifndef B200_SAD16_MINBLOCKS
-// Resident CTAs per SM the 16x16 SAD kernel is register-capped for: 4 (64 registers, no spills)
-// measured 0.850 ms per 32-pair launch against 0.931 ms at 5 (48 registers, 66 B of spills).
+// Resident CTAs per SM the 16x16 SAD kernel is register-capped for: 4 (64 registers, no spills).
 #define B200_SAD16_MINBLOCKS 4
 #endif
 
@@ -385,8 +384,8 @@ __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)_
 // Stage `rows` x `row_bytes` (row_bytes multiple of 16, src and smem rows 16-byte aligned) into
 // smem.  Half-warps own rows (16 lanes x 16 bytes = one 256-byte row segment per step); each
 // thread walks its (row, vector) column with pointer increments only, three rows in flight.
-// (A per-row cp.async.bulk / UBLKCP version was measured slower: 144 small bulk copies per window
-// serialise in the copy engine and the whole CTA waits on the mbarrier - profiles/NOTES_r1.md.)
+// (A per-row cp.async.bulk / UBLKCP version needs 144 small bulk copies per window, which serialise
+// in the copy engine while the whole CTA waits on the mbarrier.)
 __device__ __forceinline__ void stage_window(uint32_t *smem, int pitch_words, const uint8_t *src,
                                              long long src_stride, int rows, int row_bytes) {
   const int vpr = row_bytes >> 4;
@@ -500,7 +499,7 @@ __device__ __forceinline__ uint32_t chunk_satd_u8(const uint32_t *wrow, int pitc
 
 // sad = tot on lane `which`, one compare + one predicated move where they stand: written as `if (lane ==
 // sidx) sad = tot` in a fully unrolled loop the compiler hoists all 32 compares out of the loop and packs
-// the predicates into a bit mask (130 instructions per 32 candidates, ncu r2j)
+// the predicates into a bit mask
 __device__ __forceinline__ void keep_if_lane(uint32_t &sad, uint32_t tot, int lane, int which) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.eq.s32 p, %1, %2;\n\t@p mov.u32 %0, %3;\n\t}"
@@ -637,7 +636,7 @@ __global__ void __launch_bounds__(SATD ? 128 : B200_SAD_THREADS, (!SATD && W >= 
             int by_tma = 0;
             if (tma_on) {
               const bool dense0 = (long long)(hi - lo) * (W * H) * 2 >= (long long)tm.box_h * tm.box_w;
-              // the box starts on a 16-byte column of the tensor (measured: any other x faults)
+              // the box starts on a 16-byte column of the tensor
               const int cx = (x0 + tm.ox[pi]) & ~15;
               const int wx = cx - tm.ox[pi];
               by_tma = dense0 && x1 - wx + W + 4 <= tm.box_w && y1 - y0 + H <= tm.box_h;
@@ -1153,7 +1152,7 @@ __global__ void __launch_bounds__(256, SATD ? B200_WARP_SATD_MINBLOCKS : 1) me_c
 // ---------------------------------------------------------------- sparse SATD lists, 8x8 chunks
 // The warp-per-block kernel above gives every thread one 8x8 chunk of one candidate and lets it
 // fetch its own 8 rows: 32 threads read 32 different places per load (32 cache lines per
-// instruction, L1 tag bound: 0.45 ms per 32-pair launch, 120 registers).  This kernel keeps the
+// instruction, L1 tag bound, 120 registers).  This kernel keeps the
 // thread-per-chunk arithmetic (no shuffles inside the transform) but separates fetching from
 // evaluating and pipelines the two across blocks.  Per warp, for the blocks b0, b1, ... it owns:
 //   header   (block position, candidate range)        loaded three blocks ahead        -> registers
@@ -1869,8 +1868,8 @@ int launch_cand_group(b200_ctx *ctx, MeArgs a, int window_hint_px, const b200_pl
     int want = env_g > 0 ? std::min(env_g, kMaxGroup) : 0;
     if (!want) {
       // the widest group (<= 12 blocks) whose window + org tiles leave room for three CTAs per SM (227 KB of
-      // shared memory, 1 KB reserved + ~5 KB static per CTA); measured on 16x16 / +-64 px, ms per 32-pair
-      // launch: 4: 0.728, 8: 0.622, 12: 0.594, 16: 0.669 (profiles/NOTES_r2.md)
+      // shared memory, 1 KB reserved + ~5 KB static per CTA); on an H100 at 400 W, 16x16 / +-64 px, ms per 32-pair
+      // launch: 4: 0.94, 8: 0.79, 12: 0.75-0.76, 16: 0.82 (profiles/sad_group_sweep_h100.jsonl)
       const size_t budget = (size_t)227 * 1024 / 3 - 6 * 1024;
       for (want = 12; want > 1; want--) {
         const size_t bw = b200_align_up((size_t)(2 * window_hint_px + want * W + 4 + 15), 16) + 16;

@@ -23,7 +23,7 @@
 #include "common.cuh"
 
 #ifndef B200_SEARCH_MINBLOCKS
-#define B200_SEARCH_MINBLOCKS 6  // CTAs of 4 warps per SM the search kernel is register-capped for (80 regs; 4/5/6 measured: 2.47/2.20/2.15 ms per 8 pairs)
+#define B200_SEARCH_MINBLOCKS 6  // CTAs of 4 warps per SM the search kernel is register-capped for (80 regs)
 #endif
 
 namespace {
@@ -118,7 +118,7 @@ template <typename T>
 __device__ __forceinline__ uint32_t word_sad(uint32_t a, uint32_t b, uint32_t acc) {
   if (sizeof(T) == 1) return sad4_acc(a, b, acc);
   // |a - b| per u16 lane = max - min (VIMNMX.U16x2 twice; max >= min per lane, so the 32-bit subtraction
-  // never borrows across lanes) - __vabsdiffu2 expands to ten instructions on sm_100
+  // never borrows across lanes) - __vabsdiffu2 expands to ten instructions
   const uint32_t d = __vmaxu2(a, b) - __vminu2(a, b);
   return acc + (d & 0xffffu) + (d >> 16);
 }

@@ -1,5 +1,5 @@
 // quantize.cu — quantize -> dequantize -> transform-domain distortion for batches of transform
-// blocks (sm_100a): the steps of encode_tx_block that follow the forward transform
+// blocks (sm_90a): the steps of encode_tx_block that follow the forward transform
 // (src/encoder.rs:1556-1655).
 //
 //   QuantizationContext::update / quantize   src/quantize/mod.rs:219-361

@@ -1,4 +1,4 @@
-// rd_cost.cu — the one floating-point value on the RDO path (sm_100a).
+// rd_cost.cu — the one floating-point value on the RDO path (sm_90a).
 //
 //   compute_rd_cost   src/rdo.rs:718-723
 //       rate_in_bits = (rate as f64) / ((1 << OD_BITRES) as f64)          OD_BITRES = 3, ec.rs:25

@@ -1,4 +1,4 @@
-// rdo_dist.cu — the RDO distortion kernels of rav1e for batches of blocks (sm_100a).
+// rdo_dist.cu — the RDO distortion kernels of rav1e for batches of blocks (sm_90a).
 //
 //   get_weighted_sse   src/dist.rs:234-283   (asm: rav1e_weighted_sse_{W}x{H}, asm/x86/dist/sse.rs:18-35)
 //   cdef_dist_kernel   src/dist.rs:302-372   (asm: rav1e_cdef_dist_kernel_{W}x{H}, asm/x86/dist/cdef_dist.rs:18-52)

@@ -1,4 +1,4 @@
-// subpel_rdo.cu — sub-pel refinement fused with the winner's residual and forward transform (sm_100a):
+// subpel_rdo.cu — sub-pel refinement fused with the winner's residual and forward transform (sm_90a):
 // BASELINE configs[3] "speed-2 inter RDO (mc subpel + SATD + fwd-txfm fused)".
 //
 //   get_subpel_mv_rd           src/me.rs:1411-1442   (per candidate: predict_inter_single -> compute_mv_rd)

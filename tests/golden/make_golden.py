@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Extracts the reference's own known-answer vectors for the hot path into
-tests/golden/reference_kats.json (run by hand in the build container; needs /root/reference).
+tests/golden/reference_kats.json (run by hand: `python tests/golden/make_golden.py RAV1E_CHECKOUT`).
 
 Sources (xiph/rav1e @ 564ae3b):
   src/dist.rs:418-441     get_sad_same_inner   (w, h, SAD)  on the closed-form planes of :384-413
@@ -18,14 +18,15 @@ Sources (xiph/rav1e @ 564ae3b):
                                bytes and sha256 of each; the oracle and the CUDA side regenerate
                                them from their rule)
   tests/small_input.y4m   BASELINE config 0's input: the luma planes of its 5 frames (64x64, 8 bit)
-                          -> tests/golden/small_input_luma.npy
+                          -> tests/golden/small_input_luma.npy (the file itself: tests/golden/small_input.y4m)
 The Rust test code is parsed textually; nothing is executed (no rustc in this image).
 """
 import json
 import os
 import re
+import sys
 
-REF = "/root/reference/src"
+REF = os.path.join(sys.argv[1] if len(sys.argv) > 1 else "rav1e", "src")
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "reference_kats.json")
 
 

@@ -1,5 +1,5 @@
 """bench.py's reference arm runs anywhere (it times the CPU port in oracle/): one JSON line on stdout with the
-contract's keys, the same metric / unit / workload naming as the B200 arm, and nothing else on stdout.  Ranks
+contract's keys, the same metric / unit / workload naming as the GPU arm, and nothing else on stdout.  Ranks
 other than 0 exit without work (the driver launches the arm under torchrun at N > 1)."""
 import json
 import os

@@ -1,7 +1,6 @@
-"""The bench line's contract (driver-facing): the committed measurements of the round-2 tree
-(profiles/bench_r2_final.json at N=1, bench_r2_n2.json at N=2, written by `python bench.py` on B200s; the
-round-1 lines stay under the same checks) carry every key the contract names, with sane types and internally
-consistent numbers.  Guards the output format against accidental edits to bench.py."""
+"""The bench line's contract (driver-facing): the committed measurement of this tree (profiles/bench_h100.json,
+written by `python bench.py --gpus 1` on an H100) carries every key the contract names, with sane types and
+internally consistent numbers.  Guards the output format against accidental edits to bench.py."""
 import json
 import os
 
@@ -17,8 +16,7 @@ def load(name):
     return json.loads(lines[0])
 
 
-@pytest.mark.parametrize("name,n", [("bench_r1_final.json", 1), ("bench_r1_final_2gpu.json", 2),
-                                    ("bench_r2_final.json", 1), ("bench_r2_n2.json", 2)])
+@pytest.mark.parametrize("name,n", [("bench_h100.json", 1)])
 def test_contract_keys(name, n):
     d = load(name)
     for k in ("metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_step", "higher_is_better", "scaling",
@@ -49,14 +47,7 @@ def test_contract_keys(name, n):
     assert abs(d["value"] - units / (d["ms_per_step"] * 1e-3)) < 1e-6 * d["value"]
 
 
-@pytest.mark.parametrize("a,b", [("bench_r1_final.json", "bench_r1_final_2gpu.json"),
-                                 ("bench_r2_final.json", "bench_r2_n2.json")])
-def test_two_gpus_scale_weakly(a, b):
-    one, two = load(a), load(b)
-    assert 1.7 < two["value"] / one["value"] <= 2.05
-
-
-@pytest.mark.parametrize("name,n", [("bench_r2_final.json", 1), ("bench_r2_n2.json", 2)])
+@pytest.mark.parametrize("name,n", [("bench_h100.json", 1)])
 def test_strong_scaling_object(name, n):
     """auto mode carries the 4K tile workload (BASELINE configs[4]) beside the headline: whole-job units over
     the max-over-ranks step time, total work independent of N"""
@@ -66,11 +57,3 @@ def test_strong_scaling_object(name, n):
     assert abs(t["value"] - units / (t["ms_per_step"] * 1e-3)) < 1e-6 * t["value"]
     assert set(t["per_rank_leg_ms"]) == {"sad_cand", "satd_cand", "residual+fwd_txfm", "cdef_find_dir", "cdef_filter"}
 
-
-def test_strong_scaling_series():
-    one = load("bench_r2_final.json")["strong_scaling_4k_tiles"]
-    two = load("bench_r2_n2.json")["strong_scaling_4k_tiles"]
-    eight = load("bench_r2_tiles_n8.json")          # measured with --workload 4k-tiles (tiles as the line's metric)
-    assert eight["scaling"] == "strong" and eight["n_gpus"] == 8
-    assert two["value"] / one["value"] > 1.9
-    assert eight["value"] / one["value"] / 8 >= 0.9

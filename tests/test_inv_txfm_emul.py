@@ -21,7 +21,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 def emul(tmp_path_factory):
     out = str(tmp_path_factory.mktemp("inv_emul") / "libinvemul.so")
     nvcc = os.environ.get("NVCC") or "/usr/local/cuda/bin/nvcc"
-    subprocess.check_call([nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-O1", "-std=c++17",
+    subprocess.check_call([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O1", "-std=c++17",
                            "-ccbin", "/usr/bin/g++", "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC",
                            "-shared", "-I" + os.path.join(ROOT, "include"),
                            os.path.join(ROOT, "tests", "cpp", "inv_txfm_emul.cu"), "-o", out,

@@ -6,9 +6,9 @@ set -e
 cd "$(dirname "$0")/.."
 name=$1; src=$2; shift 2
 mkdir -p build/variants rav1e_b200/variants
-nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -lineinfo -Xcompiler -fPIC -ccbin /usr/bin/g++ \
+nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo -Xcompiler -fPIC -ccbin /usr/bin/g++ \
   --expt-relaxed-constexpr -Iinclude "$@" -c rav1e_b200/csrc/$src.cu -o build/variants/${src}_$name.o
 objs=$(ls build/obj/*.o | grep -v "/$src.o")
-nvcc -gencode arch=compute_100a,code=sm_100a -shared -ccbin /usr/bin/g++ -o rav1e_b200/variants/libb200rdo_$name.so \
+nvcc -gencode arch=compute_90a,code=sm_90a -shared -ccbin /usr/bin/g++ -o rav1e_b200/variants/libb200rdo_$name.so \
   build/variants/${src}_$name.o $objs -lcudart_static -lpthread -ldl -lrt
 echo rav1e_b200/variants/libb200rdo_$name.so

@@ -8,8 +8,8 @@
 //       elsewhere: the 8 outputs of a row are all a m16n8 tile can hold), org and -ref accumulated into the
 //       same tile; the VERTICAL pass then has to run on the s32 accumulator fragments, whose rows live in
 //       different lanes: three shfl.xor butterfly stages, then |.| and the sum.
-// Both must produce the same 32 sums.  Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o
-// satd_mma_probe satd_mma_probe.cu ; run on a B200; timings are per warp-iteration (32 chunks).
+// Both must produce the same 32 sums.  Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o
+// satd_mma_probe satd_mma_probe.cu ; run on the GPU; timings are per warp-iteration (32 chunks).
 #include <cuda_runtime.h>
 
 #include <cstdint>
@@ -155,7 +155,9 @@ __global__ void __launch_bounds__(256) probe(const uint8_t *data, int iters, uns
 }
 
 int main() {
-  const int ctas = 148 * 2, iters = 2000;
+  int sms = 0;
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+  const int ctas = sms * 2, iters = 2000;
   std::vector<uint8_t> h((size_t)ctas * 8 * 4096);
   srand(1);
   for (auto &b : h) b = (uint8_t)rand();
