@@ -60,11 +60,34 @@ def cpu_rate(fn, units):
     return units * reps / (time.perf_counter() - t0)
 
 
-def emit(name, units, unit_name, ms, bytes_per_unit, note="", cpu=None):
+def card():
+    """name and power limit of cuda:0, read now (nvidia-smi's row with the same PCI bus id)"""
+    import subprocess
+    props = torch.cuda.get_device_properties(0)
+    d = {"device": props.name, "power_limit_w": None}
+    try:
+        rows = subprocess.run(["nvidia-smi", "--query-gpu=pci.bus_id,name,power.limit", "--format=csv,noheader,nounits"],
+                              capture_output=True, text=True, timeout=30).stdout.strip().splitlines()
+    except (OSError, subprocess.SubprocessError):
+        return d
+    bus = getattr(props, "pci_bus_id", None)
+    for r in rows:
+        f = [x.strip() for x in r.split(",")]
+        if len(f) == 3 and (len(rows) == 1 or (bus is not None and int(f[0].split(":")[1], 16) == bus)):
+            d["nvidia_smi_name"] = f[1]
+            try:
+                d["power_limit_w"] = float(f[2])
+            except ValueError:
+                pass
+    return d
+
+
+def emit(name, units, unit_name, ms, bytes_per_unit, note="", cpu=None, extra=None):
     gbs = units * bytes_per_unit / (ms * 1e-3) / 1e9
     d = {"kernel": name, "units_per_launch": units, "unit": unit_name, "launch_ms": ms,
          "units_per_s": units / (ms * 1e-3), "algorithmic_bytes_per_unit": bytes_per_unit,
          "algorithmic_GBps": gbs, "frac_of_hbm_peak": gbs / PEAK, "peak_source": PEAK_SOURCE, "note": note}
+    d.update(extra or {})
     if cpu is not None:
         d["cpu_port_units_per_s"] = cpu
         d["cpu_threads"] = O.host_threads()
@@ -88,6 +111,7 @@ def main():
     stream = torch.cuda.Stream()
     torch.cuda.set_stream(stream)
     ctx = B.Context(0, use_torch_stream=True)
+    print(json.dumps(card()))
     rng = np.random.default_rng(0)
     W, H, PAD = 1920, 1080, 96
 
@@ -208,6 +232,33 @@ def main():
          ms, 128 + 4 + 4)
     ms = timed(lambda: ctx.importance_block_difference_dev(cur8, ref8, d_scr, d_mean), reps=10)
     emit("estimate_importance_block_difference 1080p 8-bit", nimp, "8x8 blocks", ms, 128)
+
+    # ---- temporal RDO (api/internal.rs:912-1230): speed 6's window (20 lookahead frames + the coded one)
+    from tests.test_oracle_temporal_rdo import oracle_importances, oracle_intra_costs, window_1080p
+    win = window_1080p()
+    oracle_intra_costs(win)
+    tplanes = [ctx.plane_from_host(im, win.pad) for im in win.imgs]
+    d_ti, d_tm = dev(win.intra), dev(win.mvs)
+    d_timp = torch.empty(len(win.imgs) * win.n_imp, dtype=torch.float32, device="cuda")
+
+    def window():
+        ctx.block_importances_dev(tplanes, 8, d_ti, d_tm, win.steps, d_timp)
+    l0 = ctx.launches
+    window()
+    nlaunch = ctx.launches - l0
+    ms = timed(window, reps=5)
+    units = len(win.steps) * win.n_imp
+    # per propagated source block: source + reference 8x8 blocks, its vector, intra cost and importance,
+    # and one read-modify-write of a destination importance (n_imp destinations per step)
+    bpu = 2 * 64 * 1 + 4 + 4 + 4 + 2 * 4
+    cpu = cpu_rate(lambda: oracle_importances(win), units)
+    emit("temporal RDO window 1080p 8-bit (block importances, 21 frames / 57 steps)", units, "propagated source blocks",
+         ms, bpu, "launch_ms = one whole window; the oracle's CPU rate is ONE thread (the propagation is serial)", cpu,
+         extra={"window_ms": ms, "launches_per_window": nlaunch,
+                "launch_count_note": "ctx launch counter: pass A, the CUB radix sort (counted once), bucket bounds, "
+                                     "one pass B per step"})
+    for p in tplanes:
+        ctx.plane_free(p)
 
     # ---- get_intra_edges for every 16x16 block of a frame x 13 modes, then the predictions from them
     eitems = np.zeros(nb * 13, B.EDGE_ITEM_DTYPE)

@@ -469,6 +469,50 @@ int b200_estimate_inter_costs_dev(b200_ctx *ctx, const b200_plane *org, const b2
 int b200_importance_block_difference_dev(b200_ctx *ctx, const b200_plane *org, const b200_plane *ref,
                                          uint64_t *d_scratch, double *d_mean);
 
+/* ---------------------------------------------------------------- temporal RDO (api/internal.rs, rdo.rs)
+ * compute_block_importances (internal.rs:1075-1230): the mbtree-style propagation of block importances
+ * backwards through the RDO lookahead window, then the distortion scales of the frame being coded and
+ * their normalisation (compute_{spatio,}temporal_scores, encoder.rs:744-777).  Importance blocks are
+ * 8x8 on the CEIL grid: w_imp = ceil(W / 8), h_imp = ceil(H / 8), n_imp = w_imp * h_imp; the intra-cost
+ * maps are b200_estimate_intra_costs_dev's floor(W / 8) x floor(H / 8) maps, read flat in rows of w_imp
+ * as the reference does (so only rows y < floor(n_intra / w_imp) propagate).  Results are bit-identical
+ * to the reference's f32 / integer arithmetic; the one exception is stated at b200_distortion_scales_dev.
+ *
+ * One propagation step = update_block_importances (internal.rs:912-1071) of frame `src` into its
+ * reference `dst`, `len` = the number of unique references of `src` (1..3), motion vectors = the map
+ * number `mv_index` of d_mvs (me_stats[2y][2x].mv of that reference, (row, col) i16 per importance block).
+ * Steps run in the order given: the reference's reverse frame order (key frames contribute none), each
+ * frame's references in ref_frames order.  Rejected with B200_ERR_ARG before anything is enqueued: a
+ * frame index outside the window, src == dst, len outside 1..3, and a step whose src is the dst of a
+ * LATER step (its importances would not be final yet). */
+typedef struct {
+  uint32_t src, dst; /* frame indices inside the window */
+  uint32_t len;      /* divisor: unique references of src */
+  uint32_t mv_index; /* which n_imp-entry vector map of d_mvs */
+} b200_imp_step;
+/* frames: HOST array of nframes source luma planes (same size and bpp; padding covers the ceil grid
+ * and wherever the vectors point, as for b200_estimate_inter_costs_dev); d_intra_costs: nframes x
+ * floor(W/8)*floor(H/8); d_importances: nframes x n_imp f32, zeroed by the call, then propagated. */
+int b200_block_importances_dev(b200_ctx *ctx, size_t nframes, const b200_plane *frames, int bit_depth,
+                               const uint32_t *d_intra_costs, const int16_t *d_mvs, size_t nsteps,
+                               const b200_imp_step *steps, float *d_importances);
+/* distortion_scale_for (rdo.rs:506-553) per importance block of `frame` (only its size is read):
+ * d_scales[i] = Q14 DistortionScale of pow((intra + imp) / intra, 1/3) (16384 where intra == 0 and for
+ * i >= n_intra, where the reference's zip stops).  The device's double pow is within 2 ULP where glibc's
+ * is within 1, so a scale can differ from the reference's only where 32768 * s lies within a few ULP of
+ * an odd integer (DESIGN §2). */
+int b200_distortion_scales_dev(b200_ctx *ctx, const b200_plane *frame, const float *d_importances,
+                               const uint32_t *d_intra_costs, uint32_t *d_scales);
+/* d_activity NULL: compute_temporal_scores (d_spatiotemporal, may be NULL, receives the scaled
+ * distortion scales); else compute_spatiotemporal_scores (d_activity = the activity scales of
+ * b200_activity_mask_dev; d_spatiotemporal required).  d_scales is scaled in place;
+ * *d_log_isqrt_mean_scale (may be NULL) = the returned inv_mean.blog64() >> 1; d_scale4x4 (may be NULL)
+ * = sse_wxh's per-4x4-chunk luma map (rdo.rs:177-224): 2*w_imp x 2*h_imp entries, rows scale4x4_stride
+ * apart, ready for b200_weighted_sse_dev. */
+int b200_temporal_scores_dev(b200_ctx *ctx, size_t w_imp, size_t h_imp, uint32_t *d_scales,
+                             const uint32_t *d_activity, uint32_t *d_spatiotemporal,
+                             int64_t *d_log_isqrt_mean_scale, uint32_t *d_scale4x4, size_t scale4x4_stride);
+
 /* ---------------------------------------------------------------- quantize chain
  * The steps of encode_tx_block after the forward transform (encoder.rs:1556-1655) for nblocks
  * transform blocks of one (tx_size, tx_type), device-resident:

@@ -53,6 +53,19 @@ class FramePipeCfg(C.Structure):
                 ("tx_size", C.c_int32), ("tx_type", C.c_int32), ("dc_quant", C.c_uint32), ("ac_quant", C.c_uint32)]
 
 
+class ImpStep(C.Structure):
+    """b200_imp_step: one update_block_importances step of the lookahead window."""
+    _fields_ = [("src", C.c_uint32), ("dst", C.c_uint32), ("len", C.c_uint32), ("mv_index", C.c_uint32)]
+
+
+def imp_steps(steps):
+    """[(src, dst, len, mv_index), ...] -> a ctypes array of ImpStep (execution order)."""
+    arr = (ImpStep * max(len(steps), 1))()
+    for k, s in enumerate(steps):
+        arr[k] = ImpStep(*[int(v) for v in s])
+    return arr
+
+
 BLOCK_DTYPE = np.dtype([("x", "<i2"), ("y", "<i2")])
 CAND_DTYPE = np.dtype([("block", "<u4"), ("mv_row", "<i2"), ("mv_col", "<i2")])
 INTRA_ITEM_DTYPE = np.dtype([("edge", "<u4"), ("ac", "<u4"), ("x", "<i2"), ("y", "<i2"),
@@ -203,6 +216,9 @@ def lib():
     L.b200_estimate_intra_costs_dev.argtypes = [vp, pp, i32, vp]
     L.b200_estimate_inter_costs_dev.argtypes = [vp, pp, pp, vp, vp, vp, vp]
     L.b200_importance_block_difference_dev.argtypes = [vp, pp, pp, vp, vp]
+    L.b200_block_importances_dev.argtypes = [vp, sz, vp, i32, vp, vp, sz, vp, vp]
+    L.b200_distortion_scales_dev.argtypes = [vp, pp, vp, vp, vp]
+    L.b200_temporal_scores_dev.argtypes = [vp, sz, sz, vp, vp, vp, vp, vp, sz]
     L.b200_get_intra_edges_dev.argtypes = [vp, pp] + [i32] * 7 + [vp, sz, vp, vp]
     L.b200_pred_cfl_ac_dev.argtypes = [vp, pp, vp, sz] + [i32] * 6 + [vp]
     _LIB = L
@@ -362,6 +378,29 @@ class Context:
     def importance_block_difference_dev(self, org, ref, d_scratch, d_mean):
         self.check(self.L.b200_importance_block_difference_dev(self.h, C.byref(org), C.byref(ref),
                                                                _dev_ptr(d_scratch), _dev_ptr(d_mean)))
+
+    # ---- temporal RDO
+    def block_importances_dev(self, frames, bit_depth, d_intra_costs, d_mvs, steps, d_importances):
+        """frames: list of Plane (the window's source luma); steps: [(src, dst, len, mv_index), ...] in
+        execution order; d_importances: len(frames) x ceil(W/8)*ceil(H/8) f32, zeroed then propagated."""
+        arr = (Plane * len(frames))()
+        for k, p in enumerate(frames):
+            C.memmove(C.byref(arr[k]), C.byref(p), C.sizeof(Plane))
+        st = imp_steps(steps)
+        self.check(self.L.b200_block_importances_dev(self.h, len(frames), C.addressof(arr), bit_depth,
+                                                     _dev_ptr(d_intra_costs), _dev_ptr(d_mvs), len(steps),
+                                                     C.addressof(st), _dev_ptr(d_importances)))
+
+    def distortion_scales_dev(self, frame, d_importances, d_intra_costs, d_scales):
+        self.check(self.L.b200_distortion_scales_dev(self.h, C.byref(frame), _dev_ptr(d_importances),
+                                                     _dev_ptr(d_intra_costs), _dev_ptr(d_scales)))
+
+    def temporal_scores_dev(self, w_imp, h_imp, d_scales, d_activity=None, d_spatiotemporal=None,
+                            d_log_isqrt_mean_scale=None, d_scale4x4=None, scale4x4_stride=0):
+        """d_activity None: compute_temporal_scores, else compute_spatiotemporal_scores (include/b200rdo.h)."""
+        self.check(self.L.b200_temporal_scores_dev(self.h, w_imp, h_imp, _dev_ptr(d_scales), _dev_ptr(d_activity),
+                                                   _dev_ptr(d_spatiotemporal), _dev_ptr(d_log_isqrt_mean_scale),
+                                                   _dev_ptr(d_scale4x4), scale4x4_stride))
 
     # ---- RDO cost
     def compute_rd_cost_dev(self, lam, d_rate, d_dist, n, d_cost=None, d_offsets=None, ngroups=0, d_best=None):
