@@ -163,8 +163,10 @@ typedef struct {
  *   candidates (the winner's index inside its block is packed into 24 bits).
  * Outputs (each may be NULL): d_sad[ncands], d_cost[ncands], d_best[nblocks].
  * Padding contract (the reference's, frame/mod.rs:22-23 + me.rs:339-362): candidates are accepted
- * up to get_mv_range's border, 16 + block size pixels outside the frame, so both planes must be
- * readable that far (b200_plane.pad); nothing checks it per candidate. */
+ * up to get_mv_range's border, 16 + block size pixels outside the 8-aligned frame (4 * frame_w_in_b
+ * x 4 * frame_h_in_b, which exceeds width x height when they are not multiples of 8), so both planes
+ * must be readable that far: pad >= 4 * frame_w_in_b - width + 16 + w, and likewise for y
+ * (b200_plane.pad); nothing checks it per candidate. */
 int b200_me_candidates_dev(b200_ctx *ctx, const b200_plane *cur, const b200_plane *ref,
                            const b200_block *d_blocks, size_t nblocks, const b200_cand *d_cands,
                            size_t ncands, const uint32_t *d_cand_offsets, const int16_t *d_pmv,

@@ -511,7 +511,7 @@ constexpr int kCandSmemBytes = 160 * 1024;  // upper bound of the dynamic smem (
 constexpr int kMaxGroup = 16;               // blocks sharing one staged window
 constexpr int kKeyIdxBits = 24;             // packed argmin key: cost << 24 | index in block
 
-// cost < 2^39 always (256*sad <= 2^34 for 128x128x12 bit, rate <= 61, lambda < 2^32), so
+// cost < 2^39 always (256*sad <= 2^34 for 128x128x12 bit, rate <= 64, lambda < 2^32), so
 // (cost << 24 | idx) orders exactly like (cost, idx): first minimum in list order.
 __device__ __forceinline__ unsigned long long pack_key(unsigned long long cost, uint32_t idx) {
   return cost == kEmptyCost ? ~0ull : ((cost << kKeyIdxBits) | idx);

@@ -52,54 +52,65 @@ def test_percall_noncanonical_size():
         assert L.b200_get_satd(O.ptr(a), 48, O.ptr(b), 64, w, h, 1) == want
 
 
-CAND_CASES = [
-    # (w, h, dtype, bit_depth, use_satd, per_block, max_px)
-    (16, 16, np.uint8, 8, False, 40, 40),    # some candidates fall outside get_mv_range
-    (16, 16, np.uint8, 8, True, 12, 24),
-    (8, 8, np.uint8, 8, False, 30, 16),
-    (32, 32, np.uint8, 8, False, 20, 40),
-    (4, 4, np.uint8, 8, False, 9, 12),
-    (4, 8, np.uint8, 8, True, 9, 12),
-    (64, 64, np.uint8, 8, False, 6, 70),
-    (128, 128, np.uint8, 8, True, 2, 8),
-    (16, 8, np.uint8, 8, False, 17, 30),
-    (16, 12, np.uint8, 8, True, 5, 10),      # non-canonical crop: partial chunks -> SAD
-    (16, 16, np.uint16, 10, False, 25, 24),
-    (16, 16, np.uint16, 10, True, 10, 24),
-    (32, 16, np.uint16, 12, True, 7, 24),
-    (64, 64, np.uint16, 12, False, 3, 24),
-    # sparse lists (few candidates per block): the warp-per-block kernel without window staging
-    (16, 16, np.uint8, 8, True, 4, 40),
-    (16, 16, np.uint8, 8, False, 3, 40),
-    (8, 8, np.uint8, 8, True, 2, 30),
-    (32, 32, np.uint8, 8, True, 3, 64),
-    (4, 8, np.uint8, 8, True, 3, 20),
-    (64, 64, np.uint8, 8, True, 2, 60),
-    (32, 16, np.uint8, 8, False, 1, 50),
+CAND_ROWS = [
+    # (w, h, dtype, bit_depth, use_satd, per_block, max_px, kernel the dispatcher picks)
+    # dense lists: the grouped kernel stages one window per group of blocks
+    (16, 16, np.uint8, 8, False, 40, 40, "me_cand_group_u8<16, 16, false>"),  # some candidates fall outside get_mv_range
+    (16, 16, np.uint8, 8, True, 12, 24, "me_cand_group_u8<16, 16, true>"),
+    (8, 8, np.uint8, 8, False, 30, 16, "me_cand_group_u8<8, 8, false>"),
+    (32, 32, np.uint8, 8, False, 20, 40, "me_cand_group_u8<32, 32, false>"),
+    (4, 4, np.uint8, 8, False, 9, 12, "me_cand_warp_u8<4, 4, false>"),   # 9 x 16 px: a sparse list
+    (4, 8, np.uint8, 8, True, 9, 12, "me_cand_group_u8<4, 8, true>"),
+    (64, 64, np.uint8, 8, False, 6, 70, "me_cand_group_u8<64, 64, false>"),
+    (128, 128, np.uint8, 8, True, 2, 8, "me_cand_generic<unsigned char>+me_best_from_cost"),  # beyond 64x64
+    (16, 8, np.uint8, 8, False, 17, 30, "me_cand_group_u8<16, 8, false>"),
+    # non-canonical crop: partial chunks -> SAD, generic kernel
+    (16, 12, np.uint8, 8, True, 5, 10, "me_cand_generic<unsigned char>+me_best_from_cost"),
+    (16, 16, np.uint16, 10, False, 25, 24, "me_chunk_lists<unsigned short, 16, 16, false>"),
+    (16, 16, np.uint16, 10, True, 10, 24, "me_chunk_lists<unsigned short, 16, 16, true>"),
+    (32, 16, np.uint16, 12, True, 7, 24, "me_chunk_lists<unsigned short, 32, 16, true>"),
+    (64, 64, np.uint16, 12, False, 3, 24, "me_cand_generic<unsigned short>+me_best_from_cost"),
+    # sparse lists (few candidates per block), no window staging: SATD goes to the staged 8x8-chunk
+    # kernel, SAD and the SATD sizes it does not serve (4xN, more than 32 chunks) to the warp-per-block kernel
+    (16, 16, np.uint8, 8, True, 4, 40, "me_chunk_lists<unsigned char, 16, 16, true>"),
+    (16, 16, np.uint8, 8, False, 3, 40, "me_cand_warp_u8<16, 16, false>"),
+    (8, 8, np.uint8, 8, True, 2, 30, "me_chunk_lists<unsigned char, 8, 8, true>"),
+    (32, 32, np.uint8, 8, True, 3, 64, "me_chunk_lists<unsigned char, 32, 32, true>"),
+    (4, 8, np.uint8, 8, True, 3, 20, "me_cand_warp_u8<4, 8, true>"),
+    (64, 64, np.uint8, 8, True, 2, 72, "me_cand_warp_u8<64, 64, true>"),
+    # the same list with a +-60 px reach sits just above the sparse threshold: grouped kernel
+    (64, 64, np.uint8, 8, True, 2, 60, "me_cand_group_u8<64, 64, true>"),
+    (32, 16, np.uint8, 8, False, 1, 50, "me_cand_warp_u8<32, 16, false>"),
     # sparse SATD lists through the staged 8x8-chunk kernel: every block size it serves, more
     # candidates per block than one batch holds, blocks without candidates (jitter)
-    (16, 16, np.uint8, 8, True, 8, 64),
-    (16, 16, np.uint8, 8, True, 13, 90),
-    (8, 16, np.uint8, 8, True, 5, 40),
-    (16, 8, np.uint8, 8, True, 9, 60),
-    (16, 32, np.uint8, 8, True, 5, 60),
-    (32, 16, np.uint8, 8, True, 6, 60),
-    (32, 64, np.uint8, 8, True, 2, 60),
-    (64, 32, np.uint8, 8, True, 3, 70),
-    (8, 8, np.uint8, 8, True, 1, 70),
+    (16, 16, np.uint8, 8, True, 8, 64, "me_chunk_lists<unsigned char, 16, 16, true>"),
+    (16, 16, np.uint8, 8, True, 13, 90, "me_chunk_lists<unsigned char, 16, 16, true>"),
+    (8, 16, np.uint8, 8, True, 5, 40, "me_chunk_lists<unsigned char, 8, 16, true>"),
+    (16, 8, np.uint8, 8, True, 9, 60, "me_chunk_lists<unsigned char, 16, 8, true>"),
+    (16, 32, np.uint8, 8, True, 5, 60, "me_chunk_lists<unsigned char, 16, 32, true>"),
+    (32, 16, np.uint8, 8, True, 6, 60, "me_chunk_lists<unsigned char, 32, 16, true>"),
+    (32, 64, np.uint8, 8, True, 2, 60, "me_chunk_lists<unsigned char, 32, 64, true>"),
+    (64, 32, np.uint8, 8, True, 3, 70, "me_chunk_lists<unsigned char, 64, 32, true>"),
+    (8, 8, np.uint8, 8, True, 1, 70, "me_chunk_lists<unsigned char, 8, 8, true>"),
     # high bit depth through the staged chunk kernel (16-bit lanes), dense and sparse, SAD and SATD
-    (8, 8, np.uint16, 10, False, 40, 30),
-    (8, 8, np.uint16, 12, True, 3, 30),
-    (16, 16, np.uint16, 12, False, 70, 50),
-    (16, 32, np.uint16, 10, True, 6, 40),
-    (32, 32, np.uint16, 10, False, 9, 60),
-    (32, 32, np.uint16, 12, True, 2, 60),
-    (8, 16, np.uint16, 10, False, 12, 30),
+    (8, 8, np.uint16, 10, False, 40, 30, "me_chunk_lists<unsigned short, 8, 8, false>"),
+    (8, 8, np.uint16, 12, True, 3, 30, "me_chunk_lists<unsigned short, 8, 8, true>"),
+    (16, 16, np.uint16, 12, False, 70, 50, "me_chunk_lists<unsigned short, 16, 16, false>"),
+    (16, 32, np.uint16, 10, True, 6, 40, "me_chunk_lists<unsigned short, 16, 32, true>"),
+    (32, 32, np.uint16, 10, False, 9, 60, "me_chunk_lists<unsigned short, 32, 32, false>"),
+    (32, 32, np.uint16, 12, True, 2, 60, "me_chunk_lists<unsigned short, 32, 32, true>"),
+    (8, 16, np.uint16, 10, False, 12, 30, "me_chunk_lists<unsigned short, 8, 16, false>"),
 ]
+
+
+CAND_CASES = [r[:7] for r in CAND_ROWS]
+CAND_KERNEL = {r[:7]: r[7] for r in CAND_ROWS}
+assert len(CAND_KERNEL) == len(CAND_ROWS)
 
 
 @pytest.mark.parametrize("w,h,dtype,bd,use_satd,per_block,max_px", CAND_CASES)
 def test_candidate_list_matches_oracle(w, h, dtype, bd, use_satd, per_block, max_px):
+    kernel = CAND_KERNEL[(w, h, dtype, bd, use_satd, per_block, max_px)]
     W, H, PAD = 352, 288, 160
     cur, ref = G.make_planes(W, H, PAD, dtype, seed=w * 131 + h, bit_depth=bd)
     ocur, dcur = G.both_planes(cur, PAD)
@@ -116,9 +127,9 @@ def test_candidate_list_matches_oracle(w, h, dtype, bd, use_satd, per_block, max
     d_blocks, d_cands, d_offs, d_pmv = map(G.to_dev, (blocks, cands, offs, pmv))
     d_sad, d_cost = G.dev_empty(4 * len(cands)), G.dev_empty(8 * len(cands))
     d_best = G.dev_empty(16 * len(blocks))
-    c.me_candidates_dev(dcur, dref, d_blocks, len(blocks), d_cands, len(cands), p, d_offs, d_pmv,
-                        d_sad, d_cost, d_best)
-    c.synchronize()
+    launched = G.profiled_kernels(lambda: c.me_candidates_dev(dcur, dref, d_blocks, len(blocks), d_cands, len(cands),
+                                                              p, d_offs, d_pmv, d_sad, d_cost, d_best))
+    assert launched == kernel.split("+"), launched
     got_sad = G.from_dev(d_sad, np.uint32)[:len(cands)]
     got_cost = G.from_dev(d_cost, np.uint64)[:len(cands)]
     np.testing.assert_array_equal(got_sad, want_sad)
@@ -173,21 +184,32 @@ def test_candidate_list_wrong_window_hint(hint):
         c.plane_free(pl)
 
 
-MULTI_CASES = [
-    # (w, h, dtype, bit_depth, use_satd, per_block, max_px)
-    (16, 16, np.uint8, 8, False, 64, 40),     # grouped cooperative kernel
-    (16, 16, np.uint8, 8, True, 6, 30),       # warp-per-block kernel (sparse lists)
-    (8, 8, np.uint8, 8, False, 40, 16),       # grouped, thread per candidate
-    (32, 32, np.uint8, 8, True, 20, 30),
-    (16, 12, np.uint8, 8, False, 9, 12),      # non-canonical size: generic kernel, pair by pair
-    (16, 16, np.uint16, 10, False, 12, 20),   # high bit depth: generic kernel
+MULTI_ROWS = [
+    # (w, h, dtype, bit_depth, use_satd, per_block, max_px, kernels launched)
+    (16, 16, np.uint8, 8, False, 64, 40, "me_cand_group_u8<16, 16, false>"),   # grouped cooperative kernel
+    (16, 16, np.uint8, 8, False, 4, 30, "me_cand_warp_u8<16, 16, false>"),     # warp-per-block kernel (sparse lists)
+    (16, 16, np.uint8, 8, True, 4, 30, "me_chunk_lists<unsigned char, 16, 16, true>"),  # sparse SATD lists
+    # 6 SATD candidates per block over +-30 px are just dense enough for the grouped kernel
+    (16, 16, np.uint8, 8, True, 6, 30, "me_cand_group_u8<16, 16, true>"),
+    (8, 8, np.uint8, 8, False, 40, 16, "me_cand_group_u8<8, 8, false>"),       # grouped, thread per candidate
+    (32, 32, np.uint8, 8, True, 20, 30, "me_cand_group_u8<32, 32, true>"),
+    # non-canonical size: generic kernel, pair by pair, then the segmented argmin
+    (16, 12, np.uint8, 8, False, 9, 12, "me_cand_generic<unsigned char>+me_best_from_cost"),
+    (16, 16, np.uint16, 10, False, 12, 20, "me_chunk_lists<unsigned short, 16, 16, false>"),  # high bit depth
+    (64, 64, np.uint16, 12, True, 3, 20, "me_cand_generic<unsigned short>+me_best_from_cost"),  # HBD beyond 32x32
 ]
+
+
+MULTI_CASES = [r[:7] for r in MULTI_ROWS]
+MULTI_KERNEL = {r[:7]: r[7] for r in MULTI_ROWS}
+assert len(MULTI_KERNEL) == len(MULTI_ROWS)
 
 
 @pytest.mark.parametrize("w,h,dtype,bd,use_satd,per_block,max_px", MULTI_CASES)
 def test_multi_pair_launch_matches_oracle(w, h, dtype, bd, use_satd, per_block, max_px):
     """b200_me_candidates_multi_dev: several (cur, ref) pairs with different images, different
     block subsets (one of them empty) in one call == the oracle pair by pair."""
+    kernel = MULTI_KERNEL[(w, h, dtype, bd, use_satd, per_block, max_px)]
     W, H, PAD = 320, 192, 96
     grid = G.grid_blocks(W, H, w, h)
     subsets = [grid, grid[5:37], grid[:0], grid[::3].copy(), grid[-9:]]
@@ -229,9 +251,10 @@ def test_multi_pair_launch_matches_oracle(w, h, dtype, bd, use_satd, per_block, 
     p = B.me_params(w, h, W, H, lam, use_satd=use_satd, bit_depth=bd, window_hint_px=max_px)
     d_blocks, d_cands, d_offs, d_pmv = map(G.to_dev, (blocks, cands, offs, pmv))
     d_sad, d_cost, d_best = G.dev_empty(4 * nc_tot), G.dev_empty(8 * nc_tot), G.dev_empty(16 * nb_tot)
-    c.me_candidates_multi_dev(B.PlanePairs(curs, refs, block_end, cand_end), d_blocks, nb_tot,
-                              d_cands, nc_tot, p, d_offs, d_pmv, d_sad, d_cost, d_best)
-    c.synchronize()
+    pairs = B.PlanePairs(curs, refs, block_end, cand_end)
+    launched = G.profiled_kernels(lambda: c.me_candidates_multi_dev(pairs, d_blocks, nb_tot, d_cands, nc_tot, p,
+                                                                    d_offs, d_pmv, d_sad, d_cost, d_best))
+    assert set(launched) == set(kernel.split("+")), launched
     np.testing.assert_array_equal(G.from_dev(d_sad, np.uint32)[:nc_tot], want_sad)
     np.testing.assert_array_equal(G.from_dev(d_cost, np.uint64)[:nc_tot], want_cost)
     best = G.from_dev(d_best, B.ME_RESULT_DTYPE)[:nb_tot]

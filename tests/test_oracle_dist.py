@@ -103,6 +103,68 @@ def test_mv_rate_and_range():
     assert [x.value for x in r] == [-256, (480 - 4) * 32 + 256, -256, (272 - 4) * 32 + 256]
 
 
+def _i16(v):
+    v &= 0xFFFF
+    return v - 0x10000 if v & 0x8000 else v
+
+
+def _diff_to_rate(diff, allow_hp):
+    """me.rs:1516-1519 on Python integers: `diff >> 1` is i16's arithmetic shift, `d.abs()` wraps
+    for i16::MIN, and v_frame's ILog::ilog of an i16 is 16 - leading_zeros of its 16-bit pattern."""
+    d = diff if allow_hp else diff >> 1
+    return 2 * (_i16(abs(d)) & 0xFFFF).bit_length()
+
+
+def _mv_rate(a, b, allow_hp):
+    """me.rs:1512-1523: the component differences are i16 subtractions (wrapping)."""
+    return _diff_to_rate(_i16(a[0] - b[0]), allow_hp) + _diff_to_rate(_i16(a[1] - b[1]), allow_hp)
+
+
+def _mv_cost(sad, mv, pmv0, pmv1, lam, allow_hp):
+    """me.rs:1455-1460 with unbounded integers: nothing may wrap below 2^64."""
+    rate = min(_mv_rate(mv, pmv0, allow_hp), _mv_rate(mv, pmv1, allow_hp) + 1)
+    cost = 256 * sad + rate * lam
+    assert cost < 2**64
+    return cost
+
+
+EXTREME_MV = [-32768, -32767, -16385, -16384, -9, -8, -1, 0, 1, 2, 8, 16383, 16384, 32766, 32767]
+
+
+@pytest.mark.parametrize("allow_hp", [0, 1])
+def test_mv_rate_extremes_match_bigint_restatement(allow_hp):
+    """orc_get_mv_rate on every pair of extreme components, against the restatement above: i16
+    wrap of `a - b`, the i16::MIN difference (ilog 16), the arithmetic shift without hp."""
+    L = O.lib()
+    for ar in EXTREME_MV:
+        for br in EXTREME_MV:
+            a, b = (ar, -br), (br, ar)
+            assert L.orc_get_mv_rate(O.Mv(*a), O.Mv(*b), allow_hp) == _mv_rate(a, b, allow_hp), (a, b)
+    # the wrap reaches i16::MIN from both sides
+    assert _mv_rate((0, 0), (-32768, 0), 1) == 32 and _mv_rate((-1, 0), (32767, 0), 1) == 32
+    assert _mv_rate((0, 0), (-32768, -32768), 0) == 60
+
+
+@pytest.mark.parametrize("lam", [0, 1, 2**31, 2**32 - 1])
+@pytest.mark.parametrize("allow_hp", [0, 1])
+def test_mv_cost_extremes_match_bigint_restatement(lam, allow_hp):
+    """orc_mv_cost at lambdas up to 2^32 - 1 and SADs up to a 128x128 12-bit block (and u32 max):
+    rate * lambda needs 64 bits, and the largest cost stays below 2^39, the bound the device's
+    packed argmin key relies on for every SAD a block can have."""
+    L = O.lib()
+    rng = np.random.default_rng(lam % 1000 + allow_hp)
+    sads = [0, 1, 255 * 64 * 64, 4095 * 128 * 128, 2**32 - 1]
+    for _ in range(400):
+        mv, p0, p1 = [(int(rng.choice(EXTREME_MV)), int(rng.choice(EXTREME_MV))) for _ in range(3)]
+        for sad in sads:
+            want = _mv_cost(sad, mv, p0, p1, lam, allow_hp)
+            assert L.orc_mv_cost(sad, O.Mv(*mv), O.Mv(*p0), O.Mv(*p1), lam, allow_hp) == want
+            if sad <= 4095 * 128 * 128:
+                assert want < 2**39
+    worst = _mv_cost(4095 * 128 * 128, (0, 0), (-32768, -32768), (-32768, -32768), lam, 1)
+    assert worst == 256 * 4095 * 128 * 128 + 64 * lam
+
+
 def test_full_search_first_min_tiebreak():
     """me.rs:1501 strict `<`: on a flat reference every candidate ties; the first scanned
     position (y_lo, x_lo) must win when lambda = 0."""
