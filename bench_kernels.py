@@ -260,6 +260,36 @@ def main():
     for p in tplanes:
         ctx.plane_free(p)
 
+    # ---- lookahead motion vectors (me.rs:153-337): one 1080p pair, one reference slot, three levels, one tile
+    import time
+    from tests.test_oracle_lookahead_me import Params, downsample, images, oracle_motion
+    from tests.test_oracle_lookahead_me import pyramid as la_pyramid
+    la_cur, la_ref = images(W, H, 8, True, 5)
+
+    def la_dev(img):
+        lv = [img, downsample(img)]
+        lv.append(downsample(lv[1]))
+        return [ctx.plane_from_host(im, 64) for im in lv]
+    la_dc, la_dr = la_dev(la_cur), la_dev(la_ref)
+    la_oc, la_or = la_pyramid(la_cur), la_pyramid(la_ref)
+    d_st = torch.empty(8 * (W // 4) * (H // 4 + 2), dtype=torch.uint8, device="cuda")
+    for label, fs in (("speed-6 settings: no full search", 0), ("with full search", 1)):
+        lp = Params(bit_depth=8, me_lambda=16.0, full_search=fs)
+        bp = B.LookaheadMeParams(8, 0, lp.me_lambda, fs, 1, 64, 64)
+        l0 = ctx.launches
+        ctx.lookahead_motion_dev([la_dc], [la_dr], bp, d_st)
+        nlaunch = ctx.launches - l0
+        ms = timed(lambda: ctx.lookahead_motion_dev([la_dc], [la_dr], bp, d_st), reps=5)
+        t0 = time.perf_counter()
+        oracle_motion(la_oc, la_or, W, H, lp)
+        cpu_s = time.perf_counter() - t0
+        emit(f"lookahead ME 1080p 8-bit, one ref, 3 levels ({label})", 1, "frames", ms, 2 * W * H * (1 + 0.25 + 0.0625),
+             "launch_ms = one frame (refinement + one launch per anti-diagonal); smooth pattern shifted by (5, -3) px, "
+             "me_lambda 16; the oracle's CPU rate is ONE thread (the serial reference order)", 1.0 / cpu_s,
+             extra={"frame_ms": ms, "launches_per_frame": nlaunch, "oracle_ms_per_frame": cpu_s * 1e3})
+    for p in la_dc + la_dr:
+        ctx.plane_free(p)
+
     # ---- get_intra_edges for every 16x16 block of a frame x 13 modes, then the predictions from them
     eitems = np.zeros(nb * 13, B.EDGE_ITEM_DTYPE)
     eitems["po_x"], eitems["po_y"] = np.repeat(blocks["x"], 13), np.repeat(blocks["y"], 13)

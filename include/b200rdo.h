@@ -471,6 +471,49 @@ int b200_estimate_inter_costs_dev(b200_ctx *ctx, const b200_plane *org, const b2
 int b200_importance_block_difference_dev(b200_ctx *ctx, const b200_plane *org, const b200_plane *ref,
                                          uint64_t *d_scratch, double *d_mean);
 
+/* ---------------------------------------------------------------- lookahead motion (me.rs:153-337)
+ * compute_motion_vectors (api/lookahead.rs:271-284) -> estimate_tile_motion for every tile: the
+ * three-level search (64 px blocks on the quarter, 32 px on the half, 16 px on the full resolution plane,
+ * each later level refining the previous one superblock by superblock) with get_subset_predictors'
+ * predictor gathering, bit-identical to the reference's serial order.  No sub-pel stage.
+ *
+ * A pair is one (frame, reference slot); pairs are independent and share every launch.  curs / refs:
+ * HOST arrays of npairs x {full, half, quarter} planes (b200_plane_downsample_dev builds the other two),
+ * all pairs the same size and bpp.  The result d_stats is npairs grids of w_in_b x h_in_b b200_me_stats,
+ * row-major, w_in_b = 2 * ceil(width / 8), h_in_b = 2 * ceil(height / 8) (FrameMEStats): every cell is
+ * written.  The lookahead reads it at stride 2: importance block (x, y)'s vector is cell (2x, 2y), the
+ * d_mvs entry of b200_estimate_inter_costs_dev and b200_block_importances_dev; in the other direction, a
+ * frame's d_stats grid is its successor's d_prev (subset C reads LAST's final stats for the same slot, in
+ * frame coordinates).  d_prev: NULL, or npairs grids; has_prev: HOST flags per pair (required with d_prev).
+ * Tiles: the uniform grid of tile_w_sb x tile_h_sb superblocks of TilingInfo over the 8-aligned frame, the
+ * last ones cropped; predictors never cross a tile edge.
+ *
+ * Rejected with B200_ERR_ARG before anything is enqueued: plane sizes other than w x h, (w + 1) / 2 x
+ * (h + 1) / 2 and (w + 3) / 4 x (h + 3) / 4; mixed bpp or sizes; a tile size of 0; bit_depth not 8 for
+ * bpp 1 or outside 9..12 for bpp 2; me_range_scale outside 1..16; and a pad on any plane below what the mv
+ * range needs.  With W8 = width rounded up to 8 and, at resolution level s (0 full, 1 half, 2 quarter),
+ * bw = min(s == 0 ? 32 : 64, W8 + 2^s - 1) >> s (the widest block searched there: the refinement re-searches
+ * the previous level's 64 / 32 px blocks), the pad of both level-s planes must be at least
+ *   max((16 >> s) + bw, (W8 + 16) / 2^s + bw - plane width), and likewise for heights;
+ * 20 / 40 / 48 px left and top on the quarter / half / full plane.
+ *
+ * Launches: 2 + sum over the three levels of (tbx + tby - 1), tbx x tby = the first tile's blocks at that
+ * level (min(64 * tile_w_sb, W8) / block size, rounded up): one refinement launch per later level, then one
+ * per tile-local anti-diagonal.  328 for a 1080p frame in one tile. */
+typedef struct {
+  int16_t mv_row, mv_col;  /* MEStats.mv, 1/8 pel */
+  uint32_t normalized_sad; /* sad scaled to a 128x128 block */
+} b200_me_stats;
+typedef struct {
+  int32_t bit_depth, allow_high_precision_mv;
+  double me_lambda; /* fi.me_lambda; the levels' lambdas are derived as me.rs:175-176 */
+  int32_t me_allow_full_search, me_range_scale;
+  int32_t tile_w_sb, tile_h_sb; /* TilingInfo tile size in 64 px superblocks */
+} b200_lookahead_me_params;
+int b200_lookahead_motion_dev(b200_ctx *ctx, size_t npairs, const b200_plane *curs, const b200_plane *refs,
+                              const b200_lookahead_me_params *p, const b200_me_stats *d_prev,
+                              const uint8_t *has_prev, b200_me_stats *d_stats);
+
 /* ---------------------------------------------------------------- temporal RDO (api/internal.rs, rdo.rs)
  * compute_block_importances (internal.rs:1075-1230): the mbtree-style propagation of block importances
  * backwards through the RDO lookahead window, then the distortion scales of the frame being coded and

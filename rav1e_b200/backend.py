@@ -58,6 +58,16 @@ class ImpStep(C.Structure):
     _fields_ = [("src", C.c_uint32), ("dst", C.c_uint32), ("len", C.c_uint32), ("mv_index", C.c_uint32)]
 
 
+class LookaheadMeParams(C.Structure):
+    """b200_lookahead_me_params: the frame's ME settings for b200_lookahead_motion_dev."""
+    _fields_ = [("bit_depth", C.c_int32), ("allow_high_precision_mv", C.c_int32), ("me_lambda", C.c_double),
+                ("me_allow_full_search", C.c_int32), ("me_range_scale", C.c_int32),
+                ("tile_w_sb", C.c_int32), ("tile_h_sb", C.c_int32)]
+
+
+ME_STATS_DTYPE = np.dtype([("mv_row", "<i2"), ("mv_col", "<i2"), ("normalized_sad", "<u4")])
+
+
 def imp_steps(steps):
     """[(src, dst, len, mv_index), ...] -> a ctypes array of ImpStep (execution order)."""
     arr = (ImpStep * max(len(steps), 1))()
@@ -219,6 +229,7 @@ def lib():
     L.b200_block_importances_dev.argtypes = [vp, sz, vp, i32, vp, vp, sz, vp, vp]
     L.b200_distortion_scales_dev.argtypes = [vp, pp, vp, vp, vp]
     L.b200_temporal_scores_dev.argtypes = [vp, sz, sz, vp, vp, vp, vp, vp, sz]
+    L.b200_lookahead_motion_dev.argtypes = [vp, sz, vp, vp, C.POINTER(LookaheadMeParams), vp, vp, vp]
     L.b200_get_intra_edges_dev.argtypes = [vp, pp] + [i32] * 7 + [vp, sz, vp, vp]
     L.b200_pred_cfl_ac_dev.argtypes = [vp, pp, vp, sz] + [i32] * 6 + [vp]
     _LIB = L
@@ -378,6 +389,27 @@ class Context:
     def importance_block_difference_dev(self, org, ref, d_scratch, d_mean):
         self.check(self.L.b200_importance_block_difference_dev(self.h, C.byref(org), C.byref(ref),
                                                                _dev_ptr(d_scratch), _dev_ptr(d_mean)))
+
+    def lookahead_motion_dev(self, curs, refs, params, d_stats, d_prev=None, has_prev=None):
+        """compute_motion_vectors for len(curs) (frame, reference slot) pairs: curs / refs are lists of
+        (full, half, quarter) Plane triples; d_stats receives len(curs) grids of w_in_b x h_in_b
+        ME_STATS_DTYPE; d_prev (optional) holds LAST's final grids, used where has_prev[k] is true."""
+        n = len(curs)
+        assert len(refs) == n
+        arrs = []
+        for side in (curs, refs):
+            arr = (Plane * (3 * n))()
+            for k, trip in enumerate(side):
+                assert len(trip) == 3
+                for s, p in enumerate(trip):
+                    C.memmove(C.byref(arr[3 * k + s]), C.byref(p), C.sizeof(Plane))
+            arrs.append(arr)
+        flags = None
+        if has_prev is not None:
+            flags = np.ascontiguousarray(np.asarray(has_prev, np.uint8).reshape(n))
+        self.check(self.L.b200_lookahead_motion_dev(self.h, n, C.addressof(arrs[0]), C.addressof(arrs[1]),
+                                                    C.byref(params), _dev_ptr(d_prev), _np_ptr(flags),
+                                                    _dev_ptr(d_stats)))
 
     # ---- temporal RDO
     def block_importances_dev(self, frames, bit_depth, d_intra_costs, d_mvs, steps, d_importances):
