@@ -77,6 +77,8 @@ int b200_plane_unpack_internal(b200_ctx *ctx, const b200_plane *p, const void *d
 // device copy of the scan order of (tx_size, tx_type) (scan_order.rs; owned by the context), quantize.cu
 int b200_scan_table_internal(b200_ctx *ctx, int tx_size, int tx_type, const uint16_t **d_scan);
 b200_ctx *b200_default_ctx();  // lazily created; aborts loudly if no device (no CPU fallback)
+// the plane pair and block size a motion-estimation call may take (get_sad / get_satd), me_cand.cu
+int b200_me_check_planes(b200_ctx *ctx, const b200_plane *cur, const b200_plane *ref, const b200_me_params *p);
 
 #ifdef __CUDACC__
 #define B200_HD __host__ __device__
@@ -91,6 +93,17 @@ B200_HD static inline size_t b200_align_up(size_t v, size_t a) { return (v + a -
 #define MI_SIZE 4
 #define MV_LOW (-(1 << 14))
 #define MV_UPP (1 << 14)
+
+// A plane as the kernels see it: pixel (0,0) and the row pitch, both in elements of the pixel type.
+struct PlaneView {
+  const void *data;  // pixel (0,0)
+  int stride;        // elements
+};
+
+template <typename T>
+__device__ __forceinline__ const T *px(const PlaneView &p, int x, int y) {
+  return (const T *)p.data + (long long)y * p.stride + x;
+}
 
 struct MvRange {
   int x_min, x_max, y_min, y_max;

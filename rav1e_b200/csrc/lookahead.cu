@@ -16,24 +16,18 @@
 #include <algorithm>
 
 #include "common.cuh"
-#include "satd8x8.cuh"
+#include "hadamard.cuh"
 
 namespace {
 
-using b200_satd8::satd8x8;
-
-struct View {
-  const void *data;
-  int stride;
-};
 template <typename T>
-__device__ __forceinline__ int at(const View &v, int x, int y) {
-  return (int)((const T *)v.data)[(long long)y * v.stride + x];
+__device__ __forceinline__ int at(const PlaneView &v, int x, int y) {
+  return *px<T>(v, x, y);
 }
 
 // ---- Plane::downsampled + Plane::pad
 template <typename T>
-__global__ void downsample_kernel(View src, T *dst, int dst_stride, int w, int h, int pad, int pad_w, int pad_h) {
+__global__ void downsample_kernel(PlaneView src, T *dst, int dst_stride, int w, int h, int pad, int pad_w, int pad_h) {
   const int tw = w + 2 * pad, th = h + 2 * pad;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < (long long)tw * th;
        i += (long long)gridDim.x * blockDim.x) {
@@ -48,7 +42,7 @@ __global__ void downsample_kernel(View src, T *dst, int dst_stride, int w, int h
 
 // ---- estimate_intra_costs
 template <typename T>
-__global__ void __launch_bounds__(128) intra_cost_kernel(View luma, int wb, int hb, int bit_depth, uint32_t *costs) {
+__global__ void __launch_bounds__(128) intra_cost_kernel(PlaneView luma, int wb, int hb, int bit_depth, uint32_t *costs) {
   const int n = wb * hb;
   for (int blk = blockIdx.x * blockDim.x + threadIdx.x; blk < n; blk += gridDim.x * blockDim.x) {
     const int by = blk / wb, bx = blk - by * wb, x = 8 * bx, y = 8 * by;
@@ -86,7 +80,7 @@ __global__ void __launch_bounds__(128) intra_cost_kernel(View luma, int wb, int 
 
 // ---- estimate_inter_costs: SATD(org block, reference block displaced by the block's mv)
 template <typename T>
-__global__ void __launch_bounds__(128) inter_cost_kernel(View org, View ref, int wb, int hb, const short *mvs,
+__global__ void __launch_bounds__(128) inter_cost_kernel(PlaneView org, PlaneView ref, int wb, int hb, const short *mvs,
                                                          uint32_t *costs, unsigned long long *total) {
   const int n = wb * hb;
   unsigned long long mine = 0;
@@ -110,7 +104,7 @@ __global__ void __launch_bounds__(128) inter_cost_kernel(View org, View ref, int
 
 // ---- estimate_importance_block_difference
 template <typename T>
-__global__ void __launch_bounds__(128) imp_diff_kernel(View org, View ref, int wb, int hb, unsigned long long *total) {
+__global__ void __launch_bounds__(128) imp_diff_kernel(PlaneView org, PlaneView ref, int wb, int hb, unsigned long long *total) {
   const int n = wb * hb;
   unsigned long long mine = 0;
   for (int blk = blockIdx.x * blockDim.x + threadIdx.x; blk < n; blk += gridDim.x * blockDim.x) {
@@ -163,7 +157,7 @@ extern "C" int b200_plane_downsample_dev(b200_ctx *ctx, const b200_plane *src, c
   B200_CUDA(ctx, cudaSetDevice(ctx->device));
   const long long total = (long long)(w + 2 * dst->pad) * (h + 2 * dst->pad);
   const int grid = (int)std::min<long long>((total + 255) / 256, (long long)ctx->num_sms * 16);
-  const View s{src->data, src->stride};
+  const PlaneView s{src->data, src->stride};
   if (src->bpp == 1)
     downsample_kernel<uint8_t><<<grid, 256, 0, ctx->stream>>>(s, (uint8_t *)dst->data, dst->stride, w, h, dst->pad, pad_w, pad_h);
   else
@@ -181,7 +175,7 @@ extern "C" int b200_estimate_intra_costs_dev(b200_ctx *ctx, const b200_plane *lu
   if (wb == 0 || hb == 0) return B200_OK;
   B200_CUDA(ctx, cudaSetDevice(ctx->device));
   const int grid = std::min((wb * hb + 127) / 128, ctx->num_sms * 8);
-  const View v{luma->data, luma->stride};
+  const PlaneView v{luma->data, luma->stride};
   if (luma->bpp == 1)
     intra_cost_kernel<uint8_t><<<grid, 128, 0, ctx->stream>>>(v, wb, hb, bit_depth, d_costs);
   else
@@ -201,7 +195,7 @@ extern "C" int b200_estimate_inter_costs_dev(b200_ctx *ctx, const b200_plane *or
   B200_CUDA(ctx, cudaSetDevice(ctx->device));
   B200_CUDA(ctx, cudaMemsetAsync(d_scratch, 0, 8, ctx->stream));
   const int grid = std::min((wb * hb + 127) / 128, ctx->num_sms * 8);
-  const View o{org->data, org->stride}, r{ref->data, ref->stride};
+  const PlaneView o{org->data, org->stride}, r{ref->data, ref->stride};
   if (org->bpp == 1)
     inter_cost_kernel<uint8_t><<<grid, 128, 0, ctx->stream>>>(o, r, wb, hb, d_mvs, d_costs, (unsigned long long *)d_scratch);
   else
@@ -222,7 +216,7 @@ extern "C" int b200_importance_block_difference_dev(b200_ctx *ctx, const b200_pl
   B200_CUDA(ctx, cudaSetDevice(ctx->device));
   B200_CUDA(ctx, cudaMemsetAsync(d_scratch, 0, 8, ctx->stream));
   const int grid = std::min((wb * hb + 127) / 128, ctx->num_sms * 8);
-  const View o{org->data, org->stride}, r{ref->data, ref->stride};
+  const PlaneView o{org->data, org->stride}, r{ref->data, ref->stride};
   if (org->bpp == 1)
     imp_diff_kernel<uint8_t><<<grid, 128, 0, ctx->stream>>>(o, r, wb, hb, (unsigned long long *)d_scratch);
   else

@@ -28,7 +28,7 @@
 namespace {
 
 struct LaPair {
-  PlaneRef cur[3], ref[3];  // full, half, quarter resolution
+  PlaneView cur[3], ref[3];  // full, half, quarter resolution
   int has_prev;
 };
 

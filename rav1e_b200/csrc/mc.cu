@@ -272,7 +272,7 @@ extern "C" int b200_mc_blocks_dev(b200_ctx *ctx, const b200_plane *ref, const b2
   return launch_mc(ctx, a, ref->bpp);
 }
 
-// Internal (me_kernels.cu): one `put` prediction per candidate, luma plane, packed w x h outputs.
+// Internal (me_cand.cu): one `put` prediction per candidate, luma plane, packed w x h outputs.
 int b200_mc_cands_internal(b200_ctx *ctx, const b200_plane *ref, const b200_block *d_blocks,
                            const b200_cand *d_cands, size_t ncands, int w, int h, int mode,
                            int bit_depth, void *d_out) {

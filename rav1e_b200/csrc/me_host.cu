@@ -1,6 +1,6 @@
 // me_host.cu — host-buffer (`*_batch`) and per-call reference-signature entry points of the
 // SAD/SATD/ME path.  They copy the caller's host buffers (pinned or pageable) to a stream-
-// ordered device allocation, run the same device kernels as the `_dev` forms (me_kernels.cu) and copy results back before returning.
+// ordered device allocation, run the same device kernels as the `_dev` forms (me_cand.cu, me_full_search.cu) and copy results back before returning.
 #include "common.cuh"
 
 namespace {

@@ -35,7 +35,7 @@ constexpr int kMaxPairs = 32;
 struct SearchArgs {
   int npairs;
   uint32_t block_end[kMaxPairs];  // pair k owns blocks [block_end[k-1], block_end[k])
-  PlaneRef cur[kMaxPairs], ref[kMaxPairs];
+  PlaneView cur[kMaxPairs], ref[kMaxPairs];
   const b200_block *blocks;
   const b200_cand *preds;
   const uint32_t *subset_offsets;  // nblocks * nsubsets + 1

@@ -6,17 +6,9 @@
 #include <cuda_runtime.h>
 
 #include "common.cuh"
+#include "me_dev.cuh"
 
 namespace {
-
-constexpr unsigned long long kEmptyCost = ~0ull;  // MVCandidateRD::empty(), me.rs:139-146
-constexpr uint32_t kEmptySad = ~0u;
-
-struct PlaneRef {
-  const void *data;  // pixel (0,0)
-  int stride;        // elements
-};
-
 
 struct Best {  // MotionSearchResult (+ the index of the winner inside its candidate set)
   unsigned long long cost;
@@ -33,12 +25,6 @@ __device__ __forceinline__ Best best_empty() {
   b.col = 0;
   b.idx = 0x7fffffff;
   return b;
-}
-
-__device__ __forceinline__ uint32_t sad4_acc(uint32_t a, uint32_t b, uint32_t c) {
-  uint32_t d;
-  asm("vabsdiff4.u32.u32.u32.add %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c));
-  return d;
 }
 
 // search_pattern! tables (me.rs:944-947, :1022-1025, :1035-1038, :1153-1156), full pixels
@@ -266,7 +252,7 @@ __device__ __forceinline__ Best search_block(const BlockCtx &c, const Preds &P, 
           break;
       }
       // get_fullpel_mv_rd, me.rs:1386-1409
-      const bool inr = k < n && !(col < c.rng.x_min || col > c.rng.x_max || row < c.rng.y_min || row > c.rng.y_max);
+      const bool inr = k < n && !B200_MV_OUTSIDE(row, col, c.rng);
       uint32_t acc = kCrop ? crop_sad<T>(c, inr ? col / 8 : 0, inr ? row / 8 : 0, sub)  // trunc toward zero
                           : partial_sad<T>(c, inr ? col / 8 : 0, inr ? row / 8 : 0, sub);
       acc += __shfl_xor_sync(0xffffffffu, acc, 1);

@@ -19,22 +19,12 @@
 
 namespace {
 
-struct PlaneRef {
-  const void *data;
-  int stride;  // elements
-};
-
-template <typename T>
-__device__ __forceinline__ const T *px(const PlaneRef &p, int x, int y) {
-  return (const T *)p.data + (long long)y * p.stride + x;
-}
-
 constexpr int kWsseShift = 8;  // GET_WEIGHTED_SSE_SHIFT, dist.rs:223
 
 // dist.rs:234-283.  scale: one Q14 DistortionScale per 4x4 chunk of the plane (chunk (cx, cy)
 // at scale[cy * scale_stride + cx]); blocks sit on 4-pixel positions.
 template <typename T>
-__global__ void __launch_bounds__(256) weighted_sse_kernel(PlaneRef a, PlaneRef b, const b200_block *blocks,
+__global__ void __launch_bounds__(256) weighted_sse_kernel(PlaneView a, PlaneView b, const b200_block *blocks,
                                                            size_t n, int w, int h, const uint32_t *scale,
                                                            long long scale_stride, unsigned long long *out) {
   const int lane = threadIdx.x & 31;
@@ -97,7 +87,7 @@ __device__ __forceinline__ uint32_t apply_ssim_boost(uint32_t input, uint32_t sv
 
 // dist.rs:302-372
 template <typename T>
-__global__ void __launch_bounds__(128) cdef_dist_kernel(PlaneRef src, PlaneRef dst, const b200_block *blocks,
+__global__ void __launch_bounds__(128) cdef_dist_kernel(PlaneView src, PlaneView dst, const b200_block *blocks,
                                                         size_t n, int w, int h, int bit_depth, uint32_t *out,
                                                         uint32_t *raw) {
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
@@ -178,7 +168,7 @@ extern "C" int b200_weighted_sse_dev(b200_ctx *ctx, const b200_plane *src1, cons
   B200_CUDA(ctx, cudaSetDevice(ctx->device));
   const int wpc = 8;
   const int grid = (int)std::min<size_t>((nblocks + wpc - 1) / wpc, (size_t)ctx->num_sms * 32);
-  PlaneRef a{src1->data, src1->stride}, b{src2->data, src2->stride};
+  PlaneView a{src1->data, src1->stride}, b{src2->data, src2->stride};
   if (src1->bpp == 1)
     weighted_sse_kernel<uint8_t><<<grid, wpc * 32, 0, ctx->stream>>>(a, b, d_blocks, nblocks, w, h, d_scale,
                                                                      (long long)scale_stride,
@@ -204,7 +194,7 @@ extern "C" int b200_cdef_dist_dev(b200_ctx *ctx, const b200_plane *src, const b2
   B200_REQUIRE(ctx, d_blocks && (d_out || d_raw), "NULL blocks / outputs");
   B200_CUDA(ctx, cudaSetDevice(ctx->device));
   const int grid = (int)std::min<size_t>((nblocks + 127) / 128, (size_t)ctx->num_sms * 32);
-  PlaneRef a{src->data, src->stride}, b{dst->data, dst->stride};
+  PlaneView a{src->data, src->stride}, b{dst->data, dst->stride};
   if (src->bpp == 1)
     cdef_dist_kernel<uint8_t><<<grid, 128, 0, ctx->stream>>>(a, b, d_blocks, nblocks, w, h, bit_depth, d_out, d_raw);
   else
@@ -295,7 +285,7 @@ __host__ __device__ __forceinline__ uint32_t variance_8x8_px(const T *src, long 
 }
 
 template <typename T>
-__global__ void __launch_bounds__(128) activity_mask_kernel(PlaneRef luma, int wb, int hb, int bit_depth,
+__global__ void __launch_bounds__(128) activity_mask_kernel(PlaneView luma, int wb, int hb, int bit_depth,
                                                             uint32_t *variances, uint32_t *scales) {
   const long long n = (long long)wb * hb;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
@@ -322,7 +312,7 @@ extern "C" int b200_activity_mask_dev(b200_ctx *ctx, const b200_plane *luma, int
   B200_CUDA(ctx, cudaSetDevice(ctx->device));
   const long long n = (long long)wb * hb;
   const int grid = (int)std::min<long long>((n + 127) / 128, (long long)ctx->num_sms * 32);
-  PlaneRef p{luma->data, luma->stride};
+  PlaneView p{luma->data, luma->stride};
   if (luma->bpp == 1)
     activity_mask_kernel<uint8_t><<<grid, 128, 0, ctx->stream>>>(p, wb, hb, bit_depth, d_variances, d_scales);
   else

@@ -24,11 +24,9 @@
 
 #include "fwd_txfm_dev.cuh"
 #include "mc_dev.cuh"
+#include "me_dev.cuh"
 
 namespace {
-
-constexpr unsigned long long kEmptyCost = ~0ull;
-constexpr uint32_t kEmptySad = ~0u;
 
 struct SrdoArgs {
   const void *cur, *ref;
@@ -51,12 +49,6 @@ struct SrdoArgs {
   int smem_per_warp, pred_off;  // bytes: a warp's slice, and where its two prediction buffers start
 };
 
-__device__ __forceinline__ void bfly(int &a, int &b) {
-  const int s = a + b, t = a - b;
-  a = s;
-  b = t;
-}
-
 // SATD of the W x H block: 8 lanes per 8x8 chunk (lane = row), four chunks per step
 template <typename T, int W, int H>
 __device__ __forceinline__ uint32_t warp_satd(const T *org, int os, const T *pred, int lane) {
@@ -76,19 +68,7 @@ __device__ __forceinline__ uint32_t warp_satd(const T *org, int os, const T *pre
 #pragma unroll
       for (int k = 0; k < 8; k++) v[k] = (int)o[k] - (int)p[k];
     }
-    // horizontal pass in registers (dist.rs:88-121 hadamard8_1d)
-    bfly(v[0], v[1]);
-    bfly(v[2], v[3]);
-    bfly(v[4], v[5]);
-    bfly(v[6], v[7]);
-    bfly(v[0], v[2]);
-    bfly(v[1], v[3]);
-    bfly(v[4], v[6]);
-    bfly(v[5], v[7]);
-    bfly(v[0], v[4]);
-    bfly(v[1], v[5]);
-    bfly(v[2], v[6]);
-    bfly(v[3], v[7]);
+    hadamard8(v);  // horizontal pass in registers
     // vertical pass across the 8 lanes of the chunk
 #pragma unroll
     for (int s = 1; s < 8; s <<= 1) {
@@ -138,11 +118,7 @@ __global__ void __launch_bounds__(256) subpel_rdo_kernel(const __grid_constant__
     const b200_block b = a.blocks[blk];
     const uint32_t lo = a.start ? 0u : a.cand_offsets[blk], hi = a.start ? 0u : a.cand_offsets[blk + 1];
     const MvRange rng = b200_mv_range(a.w_in_b, a.h_in_b, b.x / MI_SIZE, b.y / MI_SIZE, W, H);
-    int p0r = 0, p0c = 0, p1r = 0, p1c = 0;
-    if (a.pmv) {
-      const short *p = a.pmv + 4 * blk;
-      p0r = p[0], p0c = p[1], p1r = p[2], p1c = p[3];
-    }
+    const Pmv pm = load_pmv(a.pmv, blk);
     const T *org = (const T *)a.cur + (long long)b.y * a.cur_stride + b.x;
     T *pcur = pred0, *pbest = pred1;
     unsigned long long best_cost = kEmptyCost;
@@ -151,7 +127,7 @@ __global__ void __launch_bounds__(256) subpel_rdo_kernel(const __grid_constant__
     // get_subpel_mv_rd (me.rs:1411-1442) of one vector: prediction into `pcur`, distortion, cost
     auto eval = [&](int mv_row, int mv_col, uint32_t &sad) -> unsigned long long {
       sad = kEmptySad;
-      if (mv_col < rng.x_min || mv_col > rng.x_max || mv_row < rng.y_min || mv_row > rng.y_max) return kEmptyCost;
+      if (B200_MV_OUTSIDE(mv_row, mv_col, rng)) return kEmptyCost;
       // predict.rs:284-297 get_mv_params (luma)
       const int y0 = b.y + (mv_row >> 3), x0 = b.x + (mv_col >> 3);
       const int row_frac = (int)(((unsigned)mv_row << 1) & 0xf), col_frac = (int)(((unsigned)mv_col << 1) & 0xf);
@@ -162,7 +138,7 @@ __global__ void __launch_bounds__(256) subpel_rdo_kernel(const __grid_constant__
       mc_put_warp<T, W, H>(tile, inter, pcur, xb, col_frac, yb, row_frac, a.bit_depth, lane);
       __syncwarp();
       sad = a.use_satd ? warp_satd<T, W, H>(org, a.cur_stride, pcur, lane) : warp_sad<T, W, H>(org, a.cur_stride, pcur, lane);
-      return b200_mv_cost(sad, mv_row, mv_col, p0r, p0c, p1r, p1c, a.lambda, a.allow_hp);
+      return b200_mv_cost(sad, mv_row, mv_col, pm.r0, pm.c0, pm.r1, pm.c1, a.lambda, a.allow_hp);
     };
     if (a.start) {
       // ---- subpel_diamond_search, me.rs:1311-1383: move to the best of the four diamond points while

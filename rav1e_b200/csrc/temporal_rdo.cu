@@ -27,27 +27,15 @@
 #include <cub/device/device_radix_sort.cuh>
 
 #include "common.cuh"
-#include "satd8x8.cuh"
+#include "hadamard.cuh"
 
 namespace {
-
-using b200_satd8::satd8x8;
 
 constexpr uint32_t DS_SHIFT = 14;
 constexpr uint32_t DS_MAX = (1u << 28) - 1;
 
-struct View {
-  const void *data;
-  int stride;
-};
-
-template <typename T>
-__device__ __forceinline__ int px(const View &v, int x, int y) {
-  return (int)((const T *)v.data)[(long long)y * v.stride + x];
-}
-
 struct StepDesc {
-  View src, dst;
+  PlaneView src, dst;
   const short *mvs;         // (row, col) per importance block of the source frame
   const uint32_t *intra;    // the source frame's intra-cost map, read flat
   const float *future;      // the source frame's importances (final when the step runs)
@@ -79,7 +67,7 @@ __global__ void __launch_bounds__(128) imp_pass_a(const StepDesc *steps, int nst
 #pragma unroll
       for (int r = 0; r < 8; r++)
 #pragma unroll
-        for (int c = 0; c < 8; c++) d[r * 8 + c] = px<T>(st.src, 8 * x + c, 8 * y + r) - px<T>(st.dst, sx + c, sy + r);
+        for (int c = 0; c < 8; c++) d[r * 8 + c] = *px<T>(st.src, 8 * x + c, 8 * y + r) - *px<T>(st.dst, sx + c, sy + r);
       satd = satd8x8(d);
       const int bx = floor_div64(rx), by = floor_div64(ry);
       f = (uint32_t)(rx - 64 * bx) | (uint32_t)(ry - 64 * by) << 8;
@@ -386,8 +374,8 @@ extern "C" int b200_block_importances_dev(b200_ctx *ctx, size_t nframes, const b
   const int rows = (int)std::min<size_t>((size_t)h_imp, n_intra / (size_t)w_imp);
   for (size_t k = 0; k < nsteps; k++) {
     const b200_imp_step &s = steps[k];
-    desc[k].src = View{frames[s.src].data, frames[s.src].stride};
-    desc[k].dst = View{frames[s.dst].data, frames[s.dst].stride};
+    desc[k].src = PlaneView{frames[s.src].data, frames[s.src].stride};
+    desc[k].dst = PlaneView{frames[s.dst].data, frames[s.dst].stride};
     desc[k].mvs = (const short *)d_mvs + (size_t)s.mv_index * 2 * n_imp;
     desc[k].intra = d_intra_costs + (size_t)s.src * n_intra;
     desc[k].future = d_importances + (size_t)s.src * n_imp;

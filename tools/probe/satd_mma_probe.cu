@@ -2,7 +2,7 @@
 // Hadamard is cast as an i8 MMA and ncu shows a win".  Stand-alone micro-benchmark (not part of the
 // library): the 8x8 SATD of 32 chunk pairs per warp, operands resident in shared memory, computed
 //   (A) the way the product kernels do: thread per chunk, horizontal pass as IDP.4A chains, vertical pass
-//       as register butterflies (me_kernels.cu, me_chunk_lists);
+//       as register butterflies (me_chunk.cu, me_chunk_lists);
 //   (B) with mma.sync.m16n8k32.s32.u8.s8: pixels as the A operand (16 rows x 32 bytes = 8 chunks, natural
 //       row-major bytes, no transposes), the +-1 Hadamard matrix of one chunk column group as B (zeros
 //       elsewhere: the 8 outputs of a row are all a m16n8 tile can hold), org and -ref accumulated into the
