@@ -16,8 +16,9 @@
 // consecutive threads).  Blocks of one call must not overlap.
 //
 // The per-thread row / column passes (inv_txfm_dev.cuh) are host+device functions:
-// tests/test_inv_txfm_emul.py replays them on the CPU against the oracle (all 160 valid pairs, 8 and 10
-// bit), tests/test_zz_inv_txfm_gpu.py checks the launch on hardware.
+// tests/test_inv_txfm_emul.py replays them on the CPU against the oracle (all 160 valid pairs, 8, 10 and
+// 12 bit, also with coefficients at the limits of their type); tests/test_zz_inv_txfm_gpu.py and
+// tests/test_tx_paths_gpu.py check the launch on hardware, the latter at the clamps and past one grid stride.
 #include "inv_txfm_dev.cuh"
 
 namespace {

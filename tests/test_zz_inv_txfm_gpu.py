@@ -1,7 +1,11 @@
 """GPU parity for the inverse transform + reconstruction: CUDA (through the C ABI) ==
-oracle/inv_txfm.c, bit exact, over every valid (TxSize, TxType) pair, 8 and 10 bit, plus the
-device-resident encode_tx_block chain (residual -> forward transform -> quantize -> dequantize ->
-inverse transform add) against the same chain of oracle functions.
+oracle/inv_txfm.c, bit exact, over every valid (TxSize, TxType) pair at 8 and 10 bit with realistic
+(quantized) coefficients, plus the device-resident encode_tx_block chain (residual -> forward transform
+-> quantize -> dequantize -> inverse transform add) against the same chain of oracle functions, and the
+fused encode kernel against the three separate steps at 11 (size, type, bit depth) points.
+
+12 bit, coefficients at the clamps and type limits, every pair of the fused encode kernel against the
+oracle and the grid-stride loops are covered by tests/test_tx_paths_gpu.py.
 """
 import numpy as np
 import pytest
