@@ -106,12 +106,134 @@ def grid_blocks(w, h, bw, bh):
     return b
 
 
+def host_diamond(ctx, cur, ref, d_blocks, nb, start, p, mode, allow_hp):
+    """subpel_diamond_search (me.rs:1311-1383) as a caller without b200_subpel_search_dev runs it: the four
+    diamond points of every block still searching go through one b200_me_subpel_candidates_dev launch per
+    step, and the per-block first minimum comes back to the host, which moves the centres or halves the
+    radii.  Returns the final results and the number of steps."""
+    pattern = np.array([(1, 0), (0, 1), (-1, 0), (0, -1)])
+    res = start.copy()
+    radius = np.full(nb, 2)
+    end = 0 if allow_hp else 1
+    active = np.ones(nb, bool)
+    d_best = torch.empty(nb * 16, dtype=torch.uint8, device="cuda")
+    steps = 0
+    while active.any():
+        idx = np.nonzero(active)[0]
+        sh = radius[idx][:, None]
+        rows = res["mv_row"][idx].astype(np.int64)[:, None] + (pattern[None, :, 0] << sh)
+        cols = res["mv_col"][idx].astype(np.int64)[:, None] + (pattern[None, :, 1] << sh)
+        cands = np.zeros(4 * len(idx), B.CAND_DTYPE)
+        cands["block"] = np.repeat(idx, 4)
+        cands["mv_row"] = ((rows.reshape(-1) + 32768) % 65536 - 32768).astype(np.int16)
+        cands["mv_col"] = ((cols.reshape(-1) + 32768) % 65536 - 32768).astype(np.int16)
+        counts = np.zeros(nb, np.int64)
+        counts[idx] = 4
+        offs = np.zeros(nb + 1, np.uint32)
+        offs[1:] = np.cumsum(counts)
+        ctx.me_subpel_candidates_dev(cur, ref, d_blocks, nb, dev(cands), len(cands), p, mode, dev(offs), None, None,
+                                     None, d_best)
+        best = d_best.cpu().numpy().view(B.ME_RESULT_DTYPE)[idx]
+        better = best["cost"] < res["cost"][idx]
+        res[idx[better]] = best[better]
+        stay = idx[~better]
+        active[stay[radius[stay] == end]] = False
+        radius[stay[radius[stay] != end]] -= 1
+        steps += 1
+    return res, steps
+
+
+def subpel_sizes(ctx):
+    """b200_subpel_search_dev (diamond search + SATD + the winner's DCT_DCT) on a 1080p pair at sizes with a
+    side of 64, a control (8x8) and a size below 8 (4x8), 8 and 10 bit, next to the host-driven loop over
+    b200_me_subpel_candidates_dev + b200_mc_blocks_dev + b200_fwd_txfm_pred_dev that computes the same."""
+    import time
+    from scipy.ndimage import uniform_filter
+    rng = np.random.default_rng(12)
+    W, H, PAD = 1920, 1080, 160
+    base = uniform_filter(rng.integers(0, 256, (H + 64, W + 64)).astype(np.float32), 7)
+    base = (base - base.min()) / (base.max() - base.min())
+    for bd in (8, 10):
+        maxv = (1 << bd) - 1
+        dtype = np.uint8 if bd == 8 else np.uint16
+        ref_img = np.rint(base[32:32 + H, 32:32 + W] * maxv).astype(dtype)
+        # the current frame: the reference moved by (+5.5, -3) px, plus noise
+        mov = (base[29:29 + H, 37:37 + W] + base[29:29 + H, 38:38 + W]) / 2 * maxv
+        cur_img = np.clip(np.rint(mov + rng.normal(0, 1.5 * (maxv / 255), (H, W))), 0, maxv).astype(dtype)
+        cur, ref = ctx.plane_from_host(cur_img, PAD), ctx.plane_from_host(ref_img, PAD)
+        for (w, h) in ((64, 64), (64, 32), (16, 64), (8, 8), (4, 8)):
+            ts = TX_SIZES.index((w, h))
+            blocks = grid_blocks(W, H, w, h)
+            nb = len(blocks)
+            d_blocks = dev(blocks)
+            lam = 1200 << (bd - 8)
+            p = B.me_params(w, h, W, H, lam, use_satd=True, bit_depth=bd)
+            # full-pel starts around the true vector, SATD-scored on the device (the rescore of me.rs:596-616)
+            st = np.zeros(nb, B.CAND_DTYPE)
+            st["block"] = np.arange(nb)
+            st["mv_row"] = (-3 + rng.integers(-1, 2, nb)) * 8
+            st["mv_col"] = (5 + rng.integers(0, 2, nb)) * 8
+            d_sad = torch.empty(nb * 4, dtype=torch.uint8, device="cuda")
+            d_cost = torch.empty(nb * 8, dtype=torch.uint8, device="cuda")
+            ctx.me_candidates_dev(cur, ref, d_blocks, nb, dev(st), nb, p, None, None, d_sad, d_cost)
+            start = np.zeros(nb, B.ME_RESULT_DTYPE)
+            start["sad"] = d_sad.cpu().numpy().view(np.uint32)
+            start["cost"] = d_cost.cpu().numpy().view(np.uint64)
+            start["mv_row"], start["mv_col"] = st["mv_row"], st["mv_col"]
+            d_start = dev(start)
+            d_best = torch.empty(nb * 16, dtype=torch.uint8, device="cuda")
+            ct = torch.int16 if bd == 8 else torch.int32
+            d_coef = torch.empty(nb * w * h, dtype=ct, device="cuda")
+            ms = timed(lambda: ctx.subpel_search_dev(cur, ref, d_blocks, nb, d_start, p, d_best, 0, ts, 0, None, d_coef),
+                       reps=10)
+            fused = d_best.cpu().numpy().view(B.ME_RESULT_DTYPE)
+            fused_coef = d_coef.cpu().numpy()
+            # the host-driven loop: same starts, same results
+            d_pred = torch.empty(nb * w * h * (1 if bd == 8 else 2), dtype=torch.uint8, device="cuda")
+            d_coef2 = torch.empty(nb * w * h, dtype=ct, device="cuda")
+
+            def host_chain():
+                res, steps = host_diamond(ctx, cur, ref, d_blocks, nb, start, p, 0, False)
+                mvs = np.stack([res["mv_row"], res["mv_col"]], 1).astype(np.int16)
+                ctx.mc_blocks_dev(ref, d_blocks, dev(mvs), nb, w, h, 0, 0, bd, 0, 0, 0, d_pred)
+                ctx.fwd_txfm_pred_dev(cur, d_pred, d_blocks, nb, d_coef2, ts, 0, bd)
+                torch.cuda.synchronize()
+                return res, steps
+            host_chain()
+            reps, t0 = 0, time.perf_counter()
+            while reps < 3 or time.perf_counter() - t0 < 1.0:
+                res, steps = host_chain()
+                reps += 1
+            host_ms = (time.perf_counter() - t0) * 1e3 / reps
+            same = bool(all((res[f] == fused[f]).all() for f in ("cost", "sad", "mv_row", "mv_col"))
+                        and (d_coef2.cpu().numpy() == fused_coef).all())
+            assert same, f"{w}x{h} {bd}-bit: the host-driven loop and b200_subpel_search_dev disagree"
+            moved = int(((fused["mv_row"] != start["mv_row"]) | (fused["mv_col"] != start["mv_col"])).sum())
+            bpp = 1 if bd == 8 else 2
+            emit(f"subpel_search_dev {w}x{h} {bd}-bit (diamond + SATD + DCT_DCT, fused)", nb, "blocks", ms,
+                 (w + 7) * (h + 7) * bpp, "1080p, one launch; bytes: one source footprint per block (lower bound: "
+                 "every diamond point re-reads its footprint)",
+                 extra={"w": w, "h": h, "bit_depth": bd, "blocks_moved": moved,
+                        "library": os.path.basename(B.LIB_PATH)})
+            emit(f"host-driven diamond {w}x{h} {bd}-bit (me_subpel_candidates_dev per step + mc_blocks + "
+                 "fwd_txfm_pred)", nb, "blocks", host_ms, (w + 7) * (h + 7) * bpp,
+                 "same starts and results as the fused leg; launch_ms = whole loop by host clock, "
+                 "one device round trip per step", extra={"w": w, "h": h, "bit_depth": bd, "steps": steps,
+                                                          "same_results": same,
+                                                          "fused_speedup": host_ms / ms})
+        ctx.plane_free(cur)
+        ctx.plane_free(ref)
+
+
 def main():
     torch.cuda.set_device(0)
     stream = torch.cuda.Stream()
     torch.cuda.set_stream(stream)
     ctx = B.Context(0, use_torch_stream=True)
     print(json.dumps(card()))
+    if "--subpel-sizes" in sys.argv[1:]:
+        subpel_sizes(ctx)
+        return
     rng = np.random.default_rng(0)
     W, H, PAD = 1920, 1080, 96
 
@@ -431,6 +553,9 @@ def main():
     emit("cdef_filter 4K luma", n8, "8x8 blocks", ms, 208, cpu=cpu)
     ms = timed(lambda: ctx.cdef_filter_plane_dev(pc, pco, 1, 1, 1, W4, H4, 8, 5, None, d_dir, d_var, d_str), reps=10)
     emit("cdef_filter 4K chroma 4:2:0", n8, "4x4 blocks", ms, 8 * 8 + 16)
+
+    # ---- sub-pel diamond search at the sizes the fused kernel gained (also alone: --subpel-sizes)
+    subpel_sizes(ctx)
 
 
 if __name__ == "__main__":

@@ -234,8 +234,11 @@ int b200_me_subpel_candidates_dev(b200_ctx *ctx, const b200_plane *cur, const b2
  * still in shared memory - is subtracted from the source and run through the forward transform
  * (tx_size / tx_type; block size = transform size; tx_size < 0: no transform), like
  * b200_mc_blocks_dev + b200_fwd_txfm_pred_dev would, without any prediction touching HBM.
- * 8x8, 16x16 and 32x32 blocks; d_cand_offsets required.  d_coeffs: nblocks x w*h (i16 for 8-bit planes,
- * i32 for HBD); blocks whose candidates are all out of range get zeros. */
+ * Every AV1 block size from 4x4 to 64x64 (the 19 TxSize shapes: squares, 1:2 and 1:4 rectangles); any other
+ * params->w x h is B200_ERR_ARG before any launch.  SATD uses 4x4 Hadamard chunks when a side is 4, 8x8
+ * otherwise (get_satd).  d_cand_offsets required.  d_coeffs: nblocks x w*h (i16 for 8-bit planes, i32 for
+ * HBD) in b200_fwd_txfm_pred_dev's layout for tx_size (the 32x32-chunked order when a side is 64); blocks
+ * whose candidates are all out of range get zeros. */
 int b200_subpel_rdo_dev(b200_ctx *ctx, const b200_plane *cur, const b200_plane *ref, const b200_block *d_blocks,
                         size_t nblocks, const b200_cand *d_cands, size_t ncands, const uint32_t *d_cand_offsets,
                         const int16_t *d_pmv, const b200_me_params *params, int filter_mode, int tx_size,

@@ -100,12 +100,11 @@ __global__ void __launch_bounds__(kEncThreads) encode_tx_kernel(const __grid_con
 #pragma unroll
       for (int k = 0; k < W; k++) c[k] = tile[t * PITCH + k];
       run_1d<W>(a.tx.row_type, c);
-      constexpr int HS = H < 32 ? H : 32, WC = W < 32 ? W : 32;
-      const int off0 = (t >= 32 ? HS * WC : 0) + (t & 31);
+      const int off0 = CoefOrder<W, H>::row(t);
       CoefT *g = a.out_coef ? (CoefT *)a.out_coef + blk * (size_t)(W * H) : nullptr;
 #pragma unroll
       for (int k = 0; k < W; k++) {
-        const int idx = off0 + H * 32 * (k >= 32) + (k & 31) * HS;  // forward.rs:145-158
+        const int idx = off0 + CoefOrder<W, H>::col(k);  // forward.rs:145-158
         const CoefT v = (CoefT)round_shift_bit(c[k], a.tx.bit2);
         coef[idx] = v;
         if (g) g[idx] = v;

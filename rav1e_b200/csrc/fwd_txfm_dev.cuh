@@ -74,6 +74,16 @@ __device__ __forceinline__ void run_1d(int type, TXV (&c)[N]) {
   }
 }
 
+// Where the transform's output row t, coefficient k goes: the reference's transposed, 32x32-chunked order
+// (forward.rs:135-159; rows 32.. after the first chunk of columns, columns 32.. after all rows of the first
+// 32 columns).  dst[row(t) + col(k)]; for W, H <= 32 that is dst[k * H + t].
+template <int W, int H>
+struct CoefOrder {
+  static constexpr int HS = H < 32 ? H : 32, WC = W < 32 ? W : 32;
+  __device__ __forceinline__ static int row(int t) { return (t >= 32 ? HS * WC : 0) + (t & 31); }
+  __device__ __forceinline__ static int col(int k) { return H * 32 * (k >= 32) + (k & 31) * HS; }
+};
+
 // Everything a kernel needs to know about one (tx_size, tx_type, bit depth): set up on the host.
 struct TxSetup {
   int col_type, row_type;

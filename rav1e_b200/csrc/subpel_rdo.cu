@@ -13,10 +13,12 @@
 // formed in shared memory (the reference's four cases incl. the double-rounded H-only path and the i16
 // intermediate), measured against the source block where it sits - SAD by lanes striding the pixels,
 // SATD with 8 lanes per 8x8 chunk (lane = row: horizontal butterflies in registers, vertical ones by
-// shfl.xor) - and the best prediction so far is kept by swapping two shared buffers.  When the list is
-// exhausted the winner's prediction is still on chip: its residual goes straight through the column /
-// row passes of the forward transform (thread per column, padded transposition tile, thread per row).
+// shfl.xor), or a lane per 4x4 chunk when a side is 4 - and the best prediction so far is kept by swapping
+// two shared buffers.  When the list is exhausted the winner's prediction is still on chip: its residual
+// goes straight through the column / row passes of the forward transform (thread per column, padded
+// transposition tile, thread per row; the reference's 32x32-chunked store when a side is 64).
 // Nothing but the source footprints is read from HBM and nothing but results is written.
+// Every AV1 block size 4x4 .. 64x64 is an instantiation of the same warp-per-block kernel.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -87,6 +89,35 @@ __device__ __forceinline__ uint32_t warp_satd(const T *org, int os, const T *pre
   return (acc + 4u) >> 3;  // dist.rs:219-220 (8x8 chunks: ln = 3), one rounding for the block
 }
 
+// SATD of a block with a side below 8: 4x4 chunks (dist.rs:166-167), at most four of them (16x4, 4x16),
+// one lane per chunk with the whole 2-D Hadamard in its registers
+template <typename T, int W, int H>
+__device__ __forceinline__ uint32_t warp_satd4(const T *org, int os, const T *pred, int lane) {
+  constexpr int NCH = (W / 4) * (H / 4);
+  static_assert(NCH <= 32, "one lane per 4x4 chunk");
+  uint32_t acc = 0;
+  if (lane < NCH) {
+    const int cy = (lane / (W / 4)) * 4, cx = (lane % (W / 4)) * 4;
+    int d[16];
+#pragma unroll
+    for (int r = 0; r < 4; r++)
+#pragma unroll
+      for (int k = 0; k < 4; k++) d[r * 4 + k] = (int)org[(long long)(cy + r) * os + cx + k] - (int)pred[(cy + r) * W + cx + k];
+    acc = hadamard4x4_abs_sum(d);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  return (acc + 2u) >> 2;  // dist.rs:219-220 (4x4 chunks: ln = 2)
+}
+
+template <typename T, int W, int H>
+__device__ __forceinline__ uint32_t block_satd(const T *org, int os, const T *pred, int lane) {
+  if constexpr (W < 8 || H < 8)
+    return warp_satd4<T, W, H>(org, os, pred, lane);
+  else
+    return warp_satd<T, W, H>(org, os, pred, lane);
+}
+
 template <typename T, int W, int H>
 __device__ __forceinline__ uint32_t warp_sad(const T *org, int os, const T *pred, int lane) {
   uint32_t acc = 0;
@@ -137,7 +168,7 @@ __global__ void __launch_bounds__(256) subpel_rdo_kernel(const __grid_constant__
       __syncwarp();
       mc_put_warp<T, W, H>(tile, inter, pcur, xb, col_frac, yb, row_frac, a.bit_depth, lane);
       __syncwarp();
-      sad = a.use_satd ? warp_satd<T, W, H>(org, a.cur_stride, pcur, lane) : warp_sad<T, W, H>(org, a.cur_stride, pcur, lane);
+      sad = a.use_satd ? block_satd<T, W, H>(org, a.cur_stride, pcur, lane) : warp_sad<T, W, H>(org, a.cur_stride, pcur, lane);
       return b200_mv_cost(sad, mv_row, mv_col, pm.r0, pm.c0, pm.r1, pm.c1, a.lambda, a.allow_hp);
     };
     if (a.start) {
@@ -227,8 +258,15 @@ __global__ void __launch_bounds__(256) subpel_rdo_kernel(const __grid_constant__
 #pragma unroll
           for (int k = 0; k < W; k++) c[k] = txtile[t * PITCH + k];
           run_1d<W>(a.tx.row_type, c);
+          if constexpr (W == 64 || H == 64) {
+            CoefT *d = dst + CoefOrder<W, H>::row(t);  // the reference's 32x32-chunked order
 #pragma unroll
-          for (int k = 0; k < W; k++) dst[k * H + t] = (CoefT)round_shift_bit(c[k], a.tx.bit2);  // W, H <= 32
+            for (int k = 0; k < W; k++) d[CoefOrder<W, H>::col(k)] = (CoefT)round_shift_bit(c[k], a.tx.bit2);
+          } else {
+            // the same order: t < H <= 32 here, written as the plain transpose it reduces to
+#pragma unroll
+            for (int k = 0; k < W; k++) dst[k * H + t] = (CoefT)round_shift_bit(c[k], a.tx.bit2);
+          }
         }
       }
       __syncwarp();
@@ -272,9 +310,10 @@ static int subpel_rdo_impl(b200_ctx *ctx, const b200_plane *cur, const b200_plan
   B200_REQUIRE(ctx, cur->bpp == ref->bpp && (cur->bpp == 1 || cur->bpp == 2), "planes must share bpp (1 or 2)");
   B200_REQUIRE(ctx, (cur->bpp == 1) == (p->bit_depth == 8) && (p->bit_depth == 8 || p->bit_depth == 10 || p->bit_depth == 12),
                "bpp %d vs bit depth %d", cur->bpp, p->bit_depth);
-  B200_REQUIRE(ctx, p->w == p->h && (p->w == 8 || p->w == 16 || p->w == 32),
-               "fused sub-pel RDO serves 8x8, 16x16 and 32x32 blocks (got %dx%d): use "
-               "b200_me_subpel_candidates_dev + b200_fwd_txfm_pred_dev for other sizes", p->w, p->h);
+  int bsize = -1;  // the block sizes are the 19 transform sizes: 4x4 .. 64x64
+  for (int s = 0; s < 19; s++)
+    if (kTxW[s] == p->w && kTxH[s] == p->h) bsize = s;
+  B200_REQUIRE(ctx, bsize >= 0, "fused sub-pel RDO serves the AV1 block sizes 4x4 .. 64x64 (got %dx%d)", p->w, p->h);
   B200_REQUIRE(ctx, filter_mode >= 0 && filter_mode <= 3, "bad FilterMode %d", filter_mode);
   B200_REQUIRE(ctx, d_start != nullptr || d_cand_offsets != nullptr, "candidates must be grouped by block (CSR d_cand_offsets)");
   B200_REQUIRE(ctx, tx_size < 0 || (valid_transform(tx_size, tx_type) && kTxW[tx_size] == p->w && kTxH[tx_size] == p->h),
@@ -304,13 +343,31 @@ static int subpel_rdo_impl(b200_ctx *ctx, const b200_plane *cur, const b200_plan
   a.tx_on = tx_size >= 0;
   if (a.tx_on) a.tx = tx_setup(tx_size, tx_type, p->bit_depth);
   a.out_coef = d_coeffs;
-#define B200_SRDO(N)                                                                     \
-  if (p->w == N)                                                                         \
-    return cur->bpp == 1 ? launch_srdo<uint8_t, N, N>(ctx, a) : launch_srdo<uint16_t, N, N>(ctx, a);
-  B200_SRDO(8)
-  B200_SRDO(16)
-  B200_SRDO(32)
+  switch (bsize) {
+#define B200_SRDO(ID, W_, H_) \
+  case ID:                    \
+    return cur->bpp == 1 ? launch_srdo<uint8_t, W_, H_>(ctx, a) : launch_srdo<uint16_t, W_, H_>(ctx, a);
+    B200_SRDO(0, 4, 4)
+    B200_SRDO(1, 8, 8)
+    B200_SRDO(2, 16, 16)
+    B200_SRDO(3, 32, 32)
+    B200_SRDO(4, 64, 64)
+    B200_SRDO(5, 4, 8)
+    B200_SRDO(6, 8, 4)
+    B200_SRDO(7, 8, 16)
+    B200_SRDO(8, 16, 8)
+    B200_SRDO(9, 16, 32)
+    B200_SRDO(10, 32, 16)
+    B200_SRDO(11, 32, 64)
+    B200_SRDO(12, 64, 32)
+    B200_SRDO(13, 4, 16)
+    B200_SRDO(14, 16, 4)
+    B200_SRDO(15, 8, 32)
+    B200_SRDO(16, 32, 8)
+    B200_SRDO(17, 16, 64)
+    B200_SRDO(18, 64, 16)
 #undef B200_SRDO
+  }
   return b200_fail(ctx, B200_ERR_ARG, "unreachable block size");
 }
 
