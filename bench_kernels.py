@@ -225,6 +225,94 @@ def subpel_sizes(ctx):
         ctx.plane_free(ref)
 
 
+def intra_screen(ctx):
+    """b200_intra_mode_screen_dev over every block of a 1080p frame (one launch per size), 8 and 10 bit,
+    num_modes_rdo 3, next to the same items through b200_get_intra_edges_dev + b200_predict_intra_dev.
+    That pair is a lower bound for the composition a caller has without the fused call: it writes the 12
+    predictions per block to HBM and stops there, because the library has no SATD against packed
+    predictions.  The fused results are checked against the CPU oracle on a sample of blocks."""
+    from scipy.ndimage import uniform_filter
+    from tests.test_oracle_intra_edges import BSIZES
+    from tests.test_oracle_intra_screen import intra_mode_screen
+    rng = np.random.default_rng(21)
+    W, H, PAD, NM = 1920, 1080, 96, 3
+    base = uniform_filter(rng.integers(0, 256, (H, W)).astype(np.float32), 5)
+    base = (base - base.min()) / (base.max() - base.min())
+    angle = {1: 90, 2: 180, 3: 45, 4: 135, 5: 113, 6: 157, 7: 203, 8: 67}
+    for bd in (8, 10):
+        maxv = (1 << bd) - 1
+        dtype = np.uint8 if bd == 8 else np.uint16
+        rec_img = np.rint(base * maxv).astype(dtype)
+        src_img = np.clip(np.rint(base * maxv + rng.normal(0, 2 * (maxv / 255), (H, W))), 0, maxv).astype(dtype)
+        rec, src = ctx.plane_from_host(rec_img, PAD), ctx.plane_from_host(src_img, PAD)
+        orec, osrc = O.Plane(W, H, PAD, dtype), O.Plane(W, H, PAD, dtype)
+        orec.fill_from(rec_img)
+        osrc.fill_from(src_img)
+        for (w, h) in ((4, 4), (8, 8), (16, 16), (16, 8), (32, 32), (64, 64)):
+            xs, ys = np.arange(0, W, w), np.arange(0, H, h)          # the last row overhangs 1080
+            nb = len(xs) * len(ys)
+            items = np.zeros(nb, B.INTRA_SCREEN_ITEM_DTYPE)
+            items["x"], items["y"] = np.tile(xs, len(ys)), np.repeat(ys, len(xs))
+            items["bsize"] = BSIZES.index((w, h))
+            items["ief"] = 0
+            items["modes"] = rng.permuted(np.tile(np.arange(13, dtype=np.uint8), (nb, 1)), axis=1)
+            d_items = dev(items)
+            d_satd = torch.empty(nb * 13 * 4, dtype=torch.uint8, device="cuda")
+            d_modes = torch.empty(nb * 13, dtype=torch.uint8, device="cuda")
+            rect = (0, 0, W, H)
+            ms = timed(lambda: ctx.intra_mode_screen_dev(rec, src, rect, bd, NM, d_items, nb, d_satd, d_modes))
+            satd = d_satd.cpu().numpy().view(np.uint32).reshape(nb, 13)
+            modes = d_modes.cpu().numpy().reshape(nb, 13)
+            sample = rng.choice(nb, min(nb, 2000), replace=False)
+            want_satd, want_modes = intra_mode_screen(orec, osrc, rect, bd, NM, items[sample])
+            same = bool((satd[sample] == want_satd).all() and (modes[sample] == want_modes).all())
+            assert same, f"{w}x{h} {bd}-bit: b200_intra_mode_screen_dev disagrees with the oracle"
+            cpu = cpu_rate(lambda: intra_mode_screen(orec, osrc, rect, bd, NM, items), nb)
+            # the two-launch lower bound: one edge buffer per block, the 12 screened predictions per block
+            eit = np.zeros(nb, B.EDGE_ITEM_DTYPE)
+            eit["po_x"], eit["po_y"] = items["x"], items["y"]
+            eit["part_x"], eit["part_y"] = items["x"] >> 2, items["y"] >> 2
+            eit["bsize"], eit["tx_size"], eit["mode"], eit["enable_ief"] = items["bsize"], TX_SIZES.index((w, h)), 255, 1
+            d_eit = dev(eit)
+            d_edges = torch.empty(nb * 257 * rec_img.itemsize, dtype=torch.uint8, device="cuda")
+            d_lens = torch.empty(nb * 2, dtype=torch.uint8, device="cuda")
+            ctx.get_intra_edges_dev(rec, rect, 0, 0, bd, d_eit, nb, d_edges, d_lens)
+            lens = d_lens.cpu().numpy().reshape(nb, 2)
+            k = 13 - NM // 2
+            lm = items["modes"][:, NM // 2:].reshape(-1).astype(np.int64)
+            bx, by = np.repeat(items["x"], k), np.repeat(items["y"], k)
+            variant = np.where((bx == 0) & (by == 0), 0, np.where(by == 0, 1, np.where(bx == 0, 2, 3)))
+            mode = np.where(lm == 12, np.array([0, 2, 1, 12])[variant], lm)
+            pit = np.zeros(nb * k, B.INTRA_ITEM_DTYPE)
+            pit["edge"] = np.repeat(np.arange(nb), k)
+            pit["x"], pit["y"] = bx, by
+            pit["angle"] = [angle.get(int(m), 0) for m in mode]
+            pit["mode"], pit["variant"] = mode, variant
+            pit["ief"] = np.where((lm >= 1) & (lm <= 8), 0, -1)
+            pit["left_len"], pit["above_len"] = np.repeat(lens[:, 0], k), np.repeat(lens[:, 1], k)
+            d_pit = dev(pit)
+            d_pred = torch.empty(nb * k * w * h * rec_img.itemsize, dtype=torch.uint8, device="cuda")
+
+            def two_launch():
+                ctx.get_intra_edges_dev(rec, rect, 0, 0, bd, d_eit, nb, d_edges, d_lens)
+                ctx.predict_intra_dev(d_edges, d_pit, nb * k, None, w, h, bd, W, H, d_pred)
+            ms2 = timed(two_launch)
+            bpp = rec_img.itemsize
+            nbytes = (2 * (w + h) + 1) * bpp + w * h * bpp + 13 * 4 + 13
+            emit(f"intra_mode_screen_dev {w}x{h} {bd}-bit (edges + 12 predictions + SATD + tail sort, fused)", nb,
+                 "blocks", ms, nbytes, "1080p, num_modes_rdo 3, one launch; bytes: edge reads + source block + "
+                 "13 SATDs and 13 modes out", cpu=cpu,
+                 extra={"w": w, "h": h, "bit_depth": bd, "ms_per_frame": ms, "oracle_sample": len(sample),
+                        "same_as_oracle": same, "library": os.path.basename(B.LIB_PATH)})
+            emit(f"get_intra_edges_dev + predict_intra_dev {w}x{h} {bd}-bit (lower bound of the unfused "
+                 "composition)", nb, "blocks", ms2, nbytes + 257 * bpp + k * w * h * bpp,
+                 "same items; edges + the 12 predictions written to HBM, no SATD (the library has no SATD over "
+                 "packed predictions), so a lower bound for today's composition",
+                 extra={"w": w, "h": h, "bit_depth": bd, "ms_per_frame": ms2, "fused_speedup": ms2 / ms})
+        ctx.plane_free(rec)
+        ctx.plane_free(src)
+
+
 def main():
     torch.cuda.set_device(0)
     stream = torch.cuda.Stream()
@@ -233,6 +321,9 @@ def main():
     print(json.dumps(card()))
     if "--subpel-sizes" in sys.argv[1:]:
         subpel_sizes(ctx)
+        return
+    if "--intra-screen" in sys.argv[1:]:
+        intra_screen(ctx)
         return
     rng = np.random.default_rng(0)
     W, H, PAD = 1920, 1080, 96

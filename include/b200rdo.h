@@ -749,6 +749,41 @@ int b200_get_intra_edges_dev(b200_ctx *ctx, const b200_plane *plane, int rect_x,
 int b200_predict_intra_dev(b200_ctx *ctx, const void *d_edges, const b200_intra_item *d_items,
                            size_t nitems, const int16_t *d_ac, int w, int h, int bit_depth,
                            int plane_w, int plane_h, void *d_out);
+/* Intra mode screening, the pruning metric of intra_frame_rdo_mode_decision (rdo.rs:1433-1511) for a
+ * batch of luma blocks of one PlaneRegion (tile): per item, get_intra_edges (mode None) from `rec`,
+ * then every mode in positions num_modes_rdo / 2 .. 13 of `modes` predicted at bsize.tx_size()
+ * (partition.rs:306-328; TX_64X64 for the 128-class sizes) through PredictionMode::predict_intra
+ * (predict.rs:205-249: PredictionVariant from the tile-relative position, PAETH_PRED remapped to
+ * DC / V / H at the tile's top / left edges, intra_mode_to_angle, `ief` for directional modes only),
+ * get_satd of each prediction against `src` at the tx size, and the tail of `modes` stable-sorted by
+ * SATD (ties keep the CDF order).  One launch; the edges and the source block are staged once per
+ * block, predictions exist only in registers, `rec` is not written.
+ *
+ * `rec` / `src` with (rect_x, rect_y, rect_w, rect_h) are the tile's reconstruction and input; the
+ * region must lie inside the plane.  What may share a call is the caller's business: every block's
+ * neighbours must be final in `rec` (a whole frame in the lookahead, one wavefront of the encode
+ * loop); tiles run on their own threads and contexts (encoder.rs:3253).
+ *
+ * d_satd (nitems x 13, by PredictionMode discriminant: satds_all, 0 = not screened) and d_modes
+ * (nitems x 13: `modes` after the tail sort) may each be NULL, not both.  Rejected with B200_ERR_ARG
+ * before any launch: num_modes_rdo other than 3 / 7, a bpp that does not match bit_depth (8 / 10 /
+ * 12), rec and src of different sizes, a region outside the plane, rec->pad or src->pad below 64 (the
+ * SATD reads the whole tx block past the visible frame, as the reference does), both outputs NULL,
+ * NULL items with nitems > 0.  An item with bsize >= 22, a list entry >= 13 or repeated, or (x, y)
+ * outside the region or not a multiple of 4 gets UINT32_MAX in its 13 d_satd entries and its list
+ * copied unchanged; nothing is read or written out of bounds for it. */
+typedef struct {
+  int16_t x, y;      /* block's top-left inside the region, luma px, multiples of 4 (tile_bo.plane_offset) */
+  uint8_t bsize;     /* BlockSize 0..21 (partition.rs:130-153) */
+  int8_t ief;        /* -1: enable_intra_edge_filter off; else IntraEdgeFilterParameters::use_smooth_filter() */
+  uint8_t modes[13]; /* RAV1E_INTRA_MODES after the CDF sort (rdo.rs:1416-1428), PredictionMode discriminants */
+  uint8_t pad_;
+} b200_intra_screen_item;
+int b200_intra_mode_screen_dev(b200_ctx *ctx, const b200_plane *rec, const b200_plane *src, int rect_x, int rect_y,
+                               int rect_w, int rect_h, int bit_depth, int num_modes_rdo,
+                               const b200_intra_screen_item *d_items, size_t nitems, uint32_t *d_satd,
+                               uint8_t *d_modes);
+
 /* pred_cfl_ac (predict.rs:1020-1063; asm cfl_ac_{420,422,444}, asm/x86/predict.rs:142-186):
  * bw x bh = chroma block size; d_blocks[i] = LUMA position of block i. */
 int b200_pred_cfl_ac_dev(b200_ctx *ctx, const b200_plane *luma, const b200_block *d_blocks,

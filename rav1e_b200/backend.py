@@ -84,6 +84,8 @@ INTRA_ITEM_DTYPE = np.dtype([("edge", "<u4"), ("ac", "<u4"), ("x", "<i2"), ("y",
 EDGE_ITEM_DTYPE = np.dtype([("po_x", "<i2"), ("po_y", "<i2"), ("part_x", "<i2"), ("part_y", "<i2"), ("bx", "u1"),
                             ("by", "u1"), ("bsize", "u1"), ("tx_size", "u1"), ("mode", "u1"), ("angle_delta", "i1"),
                             ("enable_ief", "u1"), ("pad_", "u1")])
+INTRA_SCREEN_ITEM_DTYPE = np.dtype([("x", "<i2"), ("y", "<i2"), ("bsize", "u1"), ("ief", "i1"),
+                                    ("modes", "u1", (13,)), ("pad_", "u1")])
 ME_RESULT_DTYPE = np.dtype(
     {"names": ["cost", "sad", "mv_row", "mv_col"],
      "formats": ["<u8", "<u4", "<i2", "<i2"], "offsets": [0, 8, 12, 14], "itemsize": 16})
@@ -232,6 +234,7 @@ def lib():
     L.b200_lookahead_motion_dev.argtypes = [vp, sz, vp, vp, C.POINTER(LookaheadMeParams), vp, vp, vp]
     L.b200_get_intra_edges_dev.argtypes = [vp, pp] + [i32] * 7 + [vp, sz, vp, vp]
     L.b200_pred_cfl_ac_dev.argtypes = [vp, pp, vp, sz] + [i32] * 6 + [vp]
+    L.b200_intra_mode_screen_dev.argtypes = [vp, pp, pp] + [i32] * 6 + [vp, sz, vp, vp]
     _LIB = L
     return L
 
@@ -501,6 +504,13 @@ class Context:
         self.check(self.L.b200_get_intra_edges_dev(self.h, C.byref(plane), rect[0], rect[1], rect[2], rect[3], xdec,
                                                    ydec, bit_depth, _dev_ptr(d_items), n, _dev_ptr(d_edges),
                                                    _dev_ptr(d_lens)))
+
+    def intra_mode_screen_dev(self, rec, src, rect, bit_depth, num_modes_rdo, d_items, n, d_satd, d_modes):
+        """rect = (x, y, w, h) of the tile region; d_items: INTRA_SCREEN_ITEM_DTYPE on the device;
+        d_satd (n x 13 u32) and d_modes (n x 13 u8) may each be None."""
+        self.check(self.L.b200_intra_mode_screen_dev(self.h, C.byref(rec), C.byref(src), rect[0], rect[1], rect[2],
+                                                     rect[3], bit_depth, num_modes_rdo, _dev_ptr(d_items), n,
+                                                     _dev_ptr(d_satd), _dev_ptr(d_modes)))
 
     def pred_cfl_ac_dev(self, luma, d_blocks, n, bw, bh, w_pad, h_pad, xdec, ydec, d_ac):
         self.check(self.L.b200_pred_cfl_ac_dev(self.h, C.byref(luma), _dev_ptr(d_blocks), n, bw, bh,
