@@ -313,6 +313,118 @@ def intra_screen(ctx):
         ctx.plane_free(src)
 
 
+def inter_screen(ctx):
+    """b200_inter_mode_screen_dev over every block of a 1080p frame (one call per size), 8 and 10 bit, on
+    lists from the mode-list model (rdo.rs:1158-1318) for two references, one forward and one backward, with
+    include_near_mvs off as at speed 6.  Beside it, the same entries through what a caller has without the
+    fused call: b200_mc_blocks_dev put for the single entries (one launch per reference), prep of both
+    references and b200_mc_avg_dev for the compound ones.  That path writes every prediction to HBM and
+    computes no SATD, so it is a lower bound.  The fused results are checked against the CPU oracle on a
+    sample of blocks."""
+    from scipy.ndimage import uniform_filter
+    from tests.test_oracle_intra_edges import BSIZES
+    from tests.test_oracle_inter_screen import ENTRIES, build_mode_list, host_plane, inter_mode_screen, origins
+    rng = np.random.default_rng(23)
+    W, H, SPAD, RPAD = 1920, 1080, 64, 128
+    base = uniform_filter(rng.integers(0, 256, (H + 64, W + 64)).astype(np.float32), 9)
+    base = (base - base.min()) / (base.max() - base.min())
+    dy, dx = -2, 5                     # cur = ref0 moved by (dx, dy); ref1 moved the other way
+    z = (0, 0)
+    for bd in (8, 10):
+        maxv = (1 << bd) - 1
+        dtype = np.uint8 if bd == 8 else np.uint16
+        img = lambda oy, ox: np.ascontiguousarray(np.rint(base[32 + oy:32 + oy + H, 32 + ox:32 + ox + W] * maxv)
+                                                  .astype(dtype))
+        ref0_img, ref1_img = img(0, 0), img(-2 * dy, -2 * dx)
+        src_img = np.clip(img(dy, dx).astype(np.float64) + rng.normal(0, 2 * maxv / 255, (H, W)), 0, maxv).astype(dtype)
+        src, refs = ctx.plane_from_host(src_img, SPAD), [ctx.plane_from_host(r, RPAD) for r in (ref0_img, ref1_img)]
+        osrc, orefs = host_plane(src_img, SPAD), [host_plane(r, RPAD) for r in (ref0_img, ref1_img)]
+        xo, yo = origins(bd)
+        for (w, h) in ((4, 4), (8, 8), (16, 8), (16, 16), (32, 32), (64, 64)):
+            xs, ys = np.arange(0, W, w), np.arange(0, H, h)
+            nb = len(xs) * len(ys)
+            items = np.zeros(nb, B.INTER_SCREEN_ITEM_DTYPE)
+            items["x"], items["y"] = np.tile(xs, len(ys)), np.repeat(ys, len(xs))
+            items["bsize"] = BSIZES.index((w, h))
+            # per block: two-entry stacks and ME vectors near the true motion (1/8 pel), one compound entry
+            true = [(-8 * dy, -8 * dx), (8 * dy, 8 * dx)]
+            jit = rng.integers(-12, 13, (nb, 8, 2))
+            refs_a = np.full((nb, ENTRIES, 2), 0, np.uint8)
+            mvs_a = np.zeros((nb, ENTRIES, 2, 2), np.int16)
+            ns = np.zeros(nb, np.uint8)
+            for b in range(nb):
+                v = [tuple(int(t) for t in np.add(true[k % 2], jit[b, k])) for k in range(8)]
+                lst = build_mode_list(w, h, [[(v[0], z), (v[2], z)], [(v[1], z), (v[3], z)]], [v[4], v[5]], False,
+                                      True, 0, 1, [(v[6], v[7])])
+                ns[b] = len(lst)
+                for k, (_, r, mv) in enumerate(lst):
+                    refs_a[b, k] = (r[0], 0xFF if r[1] is None else r[1])
+                    mvs_a[b, k] = mv
+            items["n"] = ns
+            items["cands"]["ref"] = refs_a
+            items["cands"]["mv"] = mvs_a
+            d_items = dev(items)
+            d_satd = torch.empty(nb * ENTRIES * 4, dtype=torch.uint8, device="cuda")
+            d_order = torch.empty(nb * ENTRIES, dtype=torch.uint8, device="cuda")
+            rect = (0, 0, W, H)
+            ms = timed(lambda: ctx.inter_mode_screen_dev(src, rect, refs, xo, yo, 0, bd, d_items, nb, d_satd, d_order))
+            satd = d_satd.cpu().numpy().view(np.uint32).reshape(nb, ENTRIES)
+            order = d_order.cpu().numpy().reshape(nb, ENTRIES)
+            sample = rng.choice(nb, min(nb, 2000), replace=False)
+            want_satd, want_order = inter_mode_screen(osrc, rect, orefs, xo, yo, 0, bd, items[sample])
+            same = bool((satd[sample] == want_satd).all() and (order[sample] == want_order).all())
+            assert same, f"{w}x{h} {bd}-bit: b200_inter_mode_screen_dev disagrees with the oracle"
+            cpu_items = items[sample]
+            cpu = cpu_rate(lambda: inter_mode_screen(osrc, rect, orefs, xo, yo, 0, bd, cpu_items,
+                                                     threads=O.host_threads()), len(cpu_items))
+            # the unfused lower bound: every entry's prediction through the MC launches, written to HBM
+            n_ent = int(ns.sum())
+            bi = np.repeat(np.arange(nb), ns)
+            ki = np.concatenate([np.arange(k) for k in ns])
+            e_refs, e_mvs = refs_a[bi, ki], mvs_a[bi, ki]
+            single = e_refs[:, 1] == 0xFF
+            blk = np.zeros(n_ent, B.BLOCK_DTYPE)
+            blk["x"], blk["y"] = items["x"][bi], items["y"][bi]
+            bpp = src_img.itemsize
+            groups = []
+            for r in (0, 1):
+                m = single & (e_refs[:, 0] == r)
+                groups.append((refs[r], dev(blk[m]), dev(e_mvs[m, 0].copy()), int(m.sum()), 0))
+            comp = ~single
+            nc = int(comp.sum())
+            d_cb = dev(blk[comp])
+            groups.append((refs[0], d_cb, dev(e_mvs[comp, 0].copy()), nc, 1))
+            groups.append((refs[1], d_cb, dev(e_mvs[comp, 1].copy()), nc, 1))
+            d_out = [torch.empty(max(g[3], 1) * w * h * (bpp if g[4] == 0 else 2), dtype=torch.uint8, device="cuda")
+                     for g in groups]
+            d_avg = torch.empty(max(nc, 1) * w * h * bpp, dtype=torch.uint8, device="cuda")
+
+            def unfused():
+                for g, o in zip(groups, d_out):
+                    if g[3]:
+                        ctx.mc_blocks_dev(g[0], g[1], g[2], g[3], w, h, 0, 0, bd, 0, 0, g[4], o)
+                if nc:
+                    ctx.mc_avg_dev(d_out[2], d_out[3], d_avg, nc, w, h, bd)
+            ms2 = timed(unfused)
+            per_block = n_ent / nb
+            ncomp = nc / nb
+            fp = (w + 7) * (h + 7) * bpp
+            nbytes = 248 + w * h * bpp + (per_block + ncomp) * fp + ENTRIES * 5
+            emit(f"inter_mode_screen_dev {w}x{h} {bd}-bit (single + compound predictions + SATD + stable sort, fused)",
+                 nb, "blocks", ms, nbytes, "1080p, two references, speed-6 lists from the mode-list model; one call "
+                 "(bucketing + 3 size-class launches); bytes: item + source block + footprints + 20 SATDs / order out",
+                 cpu=cpu, extra={"w": w, "h": h, "bit_depth": bd, "ms_per_frame": ms, "entries_per_block": per_block,
+                                 "compound_per_block": ncomp, "oracle_sample": len(sample), "same_as_oracle": same,
+                                 "cpu_port_sample_blocks": len(cpu_items), "library": os.path.basename(B.LIB_PATH)})
+            emit(f"mc_blocks_dev put + prep x2 + mc_avg_dev {w}x{h} {bd}-bit (lower bound of the unfused composition)",
+                 nb, "blocks", ms2, nbytes + (per_block * w * h + ncomp * (4 * w * h)) * bpp,
+                 "same entries; predictions written to HBM and no SATD or sort (the library has no SATD over packed "
+                 "predictions), so a lower bound for today's composition",
+                 extra={"w": w, "h": h, "bit_depth": bd, "ms_per_frame": ms2, "fused_speedup": ms2 / ms})
+        for p in [src] + refs:
+            ctx.plane_free(p)
+
+
 def main():
     torch.cuda.set_device(0)
     stream = torch.cuda.Stream()
@@ -324,6 +436,9 @@ def main():
         return
     if "--intra-screen" in sys.argv[1:]:
         intra_screen(ctx)
+        return
+    if "--inter-screen" in sys.argv[1:]:
+        inter_screen(ctx)
         return
     rng = np.random.default_rng(0)
     W, H, PAD = 1920, 1080, 96

@@ -784,6 +784,52 @@ int b200_intra_mode_screen_dev(b200_ctx *ctx, const b200_plane *rec, const b200_
                                const b200_intra_screen_item *d_items, size_t nitems, uint32_t *d_satd,
                                uint8_t *d_modes);
 
+/* Inter mode screening, the SATD pruning of inter_frame_rdo_mode_decision (rdo.rs:1281-1363) for a batch
+ * of luma blocks of one PlaneRegion (tile): per item, every entry of its resolved mode list predicted at
+ * the full block size through PredictionMode::predict_inter (predict.rs:284-421): put_8tap for a single
+ * reference, prep_8tap of both references then mc_avg for a compound pair, both with FilterMode
+ * `filter_mode` (fi.default_filter) in both directions; the source position is get_mv_params', including
+ * PlaneSlice::clamp to [-xorigin, width] x [-yorigin, height] (a rav1e caller passes its luma plane's
+ * cfg.xorigin / cfg.yorigin); get_satd of each prediction against `src`; the entries stable-sorted by SATD
+ * (sort_by_key, ties keep list order).  Predictions exist only in shared memory.
+ *
+ * The mode list itself (rdo.rs:1158-1318, find_mvrefs' stacks) stays with the caller, and so do two of
+ * its quirks: rdo.rs computes and sorts the SATDs only when num_modes_rdo != the list's length (lists
+ * shorter than 9 included), and a missing reference frame (`if let Some(ref rec)`) leaves a stale
+ * prediction there; call this only for lists the reference screens, over present references.
+ *
+ * `src` with (rect_x, rect_y, rect_w, rect_h) is the tile's input and region (inside the plane);
+ * refs[0 .. nrefs) are whole reference frames (fi.rec_buffer slots, 1 <= nrefs <= 8) of src's size and
+ * bpp, addressed by the entries' `ref` indices.  Up to four launches (a validation / bucketing pass by
+ * size class, then one per class); no host synchronisation; context scratch holds the buckets.
+ *
+ * d_satd (nitems x 20, list order, UINT32_MAX at positions >= n) and d_order (nitems x 20: the stable
+ * ascending sort of entries 0 .. n by SATD followed by n .. 19, a permutation of 0 .. 19) may each be
+ * NULL, not both.  Rejected with B200_ERR_ARG before any launch: a bit depth other than 8 / 10 / 12 or a
+ * bpp that does not match it, nrefs outside 1 .. 8 or a reference whose size or bpp differs from src, a
+ * region outside the plane, filter_mode outside 0 .. 3, src->pad below 64, a negative xorigin / yorigin, a
+ * reference pad below max(xorigin, yorigin, 71) (the clamped footprint spans [-origin, size + 70]), both
+ * outputs NULL, NULL items with nitems > 0.  An item with bsize >= 22 or 128-sided (13 / 14 / 15), n > 20,
+ * a ref index >= nrefs in one of its n entries, or (x, y) outside the region or not a multiple of 4 gets
+ * UINT32_MAX in its 20 d_satd entries and the identity order; nothing is read or written out of bounds
+ * for it.  nitems == 0 launches nothing. */
+typedef struct {
+  int16_t mv[2][2]; /* mv[k] = {row, col}, 1/8 pel (MotionVector); mv[1] ignored for a single reference */
+  uint8_t ref[2];   /* index into refs[]; ref[1] = 0xFF: single reference (NONE_FRAME) */
+  uint8_t pad_[2];
+} b200_inter_screen_cand; /* 12 B */
+typedef struct {
+  int16_t x, y;  /* block's top-left inside the region, luma px, multiples of 4 */
+  uint8_t bsize; /* BlockSize 0..21 (partition.rs:130-153) */
+  uint8_t n;     /* entries used, 0..20 (ArrayVec<_, 20>, rdo.rs:1158) */
+  uint8_t pad_[2];
+  b200_inter_screen_cand cands[20];
+} b200_inter_screen_item; /* 248 B */
+int b200_inter_mode_screen_dev(b200_ctx *ctx, const b200_plane *src, int rect_x, int rect_y, int rect_w,
+                               int rect_h, const b200_plane *refs, int nrefs, int xorigin, int yorigin,
+                               int filter_mode, int bit_depth, const b200_inter_screen_item *d_items,
+                               size_t nitems, uint32_t *d_satd, uint8_t *d_order);
+
 /* pred_cfl_ac (predict.rs:1020-1063; asm cfl_ac_{420,422,444}, asm/x86/predict.rs:142-186):
  * bw x bh = chroma block size; d_blocks[i] = LUMA position of block i. */
 int b200_pred_cfl_ac_dev(b200_ctx *ctx, const b200_plane *luma, const b200_block *d_blocks,

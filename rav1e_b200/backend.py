@@ -86,6 +86,11 @@ EDGE_ITEM_DTYPE = np.dtype([("po_x", "<i2"), ("po_y", "<i2"), ("part_x", "<i2"),
                             ("enable_ief", "u1"), ("pad_", "u1")])
 INTRA_SCREEN_ITEM_DTYPE = np.dtype([("x", "<i2"), ("y", "<i2"), ("bsize", "u1"), ("ief", "i1"),
                                     ("modes", "u1", (13,)), ("pad_", "u1")])
+INTER_SCREEN_CAND_DTYPE = np.dtype([("mv", "<i2", (2, 2)), ("ref", "u1", (2,)), ("pad_", "u1", (2,))])
+INTER_SCREEN_ITEM_DTYPE = np.dtype([("x", "<i2"), ("y", "<i2"), ("bsize", "u1"), ("n", "u1"), ("pad_", "u1", (2,)),
+                                    ("cands", INTER_SCREEN_CAND_DTYPE, (20,))])
+assert INTER_SCREEN_CAND_DTYPE.itemsize == 12 and INTER_SCREEN_ITEM_DTYPE.itemsize == 248
+INTER_SCREEN_SINGLE = 0xFF   # b200_inter_screen_cand.ref[1] of a single-reference entry (NONE_FRAME)
 ME_RESULT_DTYPE = np.dtype(
     {"names": ["cost", "sad", "mv_row", "mv_col"],
      "formats": ["<u8", "<u4", "<i2", "<i2"], "offsets": [0, 8, 12, 14], "itemsize": 16})
@@ -235,6 +240,7 @@ def lib():
     L.b200_get_intra_edges_dev.argtypes = [vp, pp] + [i32] * 7 + [vp, sz, vp, vp]
     L.b200_pred_cfl_ac_dev.argtypes = [vp, pp, vp, sz] + [i32] * 6 + [vp]
     L.b200_intra_mode_screen_dev.argtypes = [vp, pp, pp] + [i32] * 6 + [vp, sz, vp, vp]
+    L.b200_inter_mode_screen_dev.argtypes = [vp, pp] + [i32] * 4 + [vp] + [i32] * 5 + [vp, sz, vp, vp]
     _LIB = L
     return L
 
@@ -511,6 +517,19 @@ class Context:
         self.check(self.L.b200_intra_mode_screen_dev(self.h, C.byref(rec), C.byref(src), rect[0], rect[1], rect[2],
                                                      rect[3], bit_depth, num_modes_rdo, _dev_ptr(d_items), n,
                                                      _dev_ptr(d_satd), _dev_ptr(d_modes)))
+
+    def inter_mode_screen_dev(self, src, rect, refs, xorigin, yorigin, filter_mode, bit_depth, d_items, n, d_satd,
+                              d_order):
+        """rect = (x, y, w, h) of the tile region; refs: a list of Plane (the entries' `ref` indices address
+        it); d_items: INTER_SCREEN_ITEM_DTYPE on the device; d_satd (n x 20 u32) and d_order (n x 20 u8) may
+        each be None."""
+        arr = (Plane * max(len(refs), 1))()
+        for k, p in enumerate(refs):
+            C.memmove(C.byref(arr[k]), C.byref(p), C.sizeof(Plane))
+        self.check(self.L.b200_inter_mode_screen_dev(self.h, C.byref(src), rect[0], rect[1], rect[2], rect[3],
+                                                     C.addressof(arr), len(refs), xorigin, yorigin, filter_mode,
+                                                     bit_depth, _dev_ptr(d_items), n, _dev_ptr(d_satd),
+                                                     _dev_ptr(d_order)))
 
     def pred_cfl_ac_dev(self, luma, d_blocks, n, bw, bh, w_pad, h_pad, xdec, ydec, d_ac):
         self.check(self.L.b200_pred_cfl_ac_dev(self.h, C.byref(luma), _dev_ptr(d_blocks), n, bw, bh,

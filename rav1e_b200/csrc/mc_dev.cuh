@@ -7,6 +7,13 @@
 // (sum + 2^(6+ib)) >> (7+ib) equals the V-only (sum + 64) >> 7; an identity V pass turns
 // round(128 * inter, 7+ib) into round(inter, ib), the H-only case's second rounding; and the i16
 // intermediate never truncates (|inter| <= 20.5 K at every bit depth).  So one code path serves all.
+//   prep_8tap  src/mc.rs:360-451 (the compound path's i16 predictions, PREP_BIAS 8192 subtracted at 10/12 bit)
+// has the same four cases with one rounding less: integer copy px << ib, V only round_shift(sum, 7-ib),
+// H only round_shift(sum, 7-ib), HV round_shift(sum, 7) over the same i16 intermediate.  The identity
+// argument holds for them too: an identity H pass gives px << ib, and then the V rounding
+// (128 * 2^ib * S' + 2^6) >> 7 equals (S' + 2^(6-ib)) >> (7-ib) for the V-only sum S' (and px << ib for the
+// copy); an identity V pass gives round(128 * inter, 7) = inter, the H-only case.  mc_prep_warp shares the H
+// pass with mc_put_warp and differs in the V rounding and the bias only.
 //
 // Arithmetic on packed words instead of one multiply per tap and pixel:
 //   H pass, 8-bit pixels : IDP.4A - four u8 pixels x four s8 taps per instruction (every tap fits s8:
@@ -85,17 +92,13 @@ __device__ __forceinline__ void mc_stage_tile(T *tile, const T *src, long long s
   }
 }
 
-// tile -> pred (W x H, packed) through the transposed i16 intermediate.  All lanes of the warp call it;
-// the caller brackets it with __syncwarp() (tile ready before, pred consumed after).
+// H pass over the H + 7 rows of the tile into the transposed i16 intermediate (mc.rs:312-327, :421-429),
+// 4 outputs per task.  The identity filter's tap (128) does not fit s8: a direction without a fraction
+// takes its closed form (see the header comment).
 template <typename T, int W, int H>
-__device__ __forceinline__ void mc_put_warp(const T *tile, short *interT, T *pred, int xbank, int col_frac, int ybank,
-                                            int row_frac, int bit_depth, int lane) {
+__device__ __forceinline__ void mc_hpass_warp(const T *tile, short *interT, const McTaps &xt, int col_frac, int ib,
+                                              int lane) {
   using L = McLayout<T, W, H>;
-  const int ib = 4 - (bit_depth == 12 ? 2 : 0);
-  const int maxv = (1 << bit_depth) - 1;
-  const McTaps xt = mc_taps(xbank, col_frac), yt = mc_taps(ybank, row_frac);
-  // ---- H pass over the H + 7 rows (mc.rs:312-327), 4 outputs per task.  The identity filter's tap (128)
-  // does not fit s8: a direction without a fraction takes its closed form (see the header comment).
   for (int task = lane; task < L::TH * (W / 4); task += 32) {
     const int r = task / (W / 4), g = task - r * (W / 4);
     int s[4];
@@ -120,6 +123,18 @@ __device__ __forceinline__ void mc_put_warp(const T *tile, short *interT, T *pre
 #pragma unroll
     for (int j = 0; j < 4; j++) interT[(4 * g + j) * L::THP + r] = (short)rshift_round(s[j], 7 - ib);  // `as i16`, mc.rs:323
   }
+}
+
+// tile -> pred (W x H, packed) through the transposed i16 intermediate.  All lanes of the warp call it;
+// the caller brackets it with __syncwarp() (tile ready before, pred consumed after).
+template <typename T, int W, int H>
+__device__ __forceinline__ void mc_put_warp(const T *tile, short *interT, T *pred, int xbank, int col_frac, int ybank,
+                                            int row_frac, int bit_depth, int lane) {
+  using L = McLayout<T, W, H>;
+  const int ib = 4 - (bit_depth == 12 ? 2 : 0);
+  const int maxv = (1 << bit_depth) - 1;
+  const McTaps xt = mc_taps(xbank, col_frac), yt = mc_taps(ybank, row_frac);
+  mc_hpass_warp<T, W, H>(tile, interT, xt, col_frac, ib, lane);
   __syncwarp();
   // ---- V pass (mc.rs:328-343): column c, rows 4q .. 4q+3
   for (int task = lane; task < W * (H / 4); task += 32) {
@@ -137,6 +152,44 @@ __device__ __forceinline__ void mc_put_warp(const T *tile, short *interT, T *pre
 #pragma unroll
     for (int j = 0; j < 4; j++) pred[(4 * q + j) * W + c] = (T)min(max(rshift_round(s[j], 7 + ib), 0), maxv);
   }
+}
+
+// tile -> tmp (W x H packed i16, prep_8tap's output, mc.rs:360-451): the same H pass, then the V pass rounded
+// by 7 instead of 7 + ib, no clamp, minus PREP_BIAS (8192 at 10 / 12 bit, mc.rs:357).  Same calling
+// convention as mc_put_warp.
+template <typename T, int W, int H>
+__device__ __forceinline__ void mc_prep_warp(const T *tile, short *interT, short *tmp, int xbank, int col_frac,
+                                             int ybank, int row_frac, int bit_depth, int lane) {
+  using L = McLayout<T, W, H>;
+  const int ib = 4 - (bit_depth == 12 ? 2 : 0);
+  const int bias = bit_depth == 8 ? 0 : 8192;
+  const McTaps xt = mc_taps(xbank, col_frac), yt = mc_taps(ybank, row_frac);
+  mc_hpass_warp<T, W, H>(tile, interT, xt, col_frac, ib, lane);
+  __syncwarp();
+  for (int task = lane; task < W * (H / 4); task += 32) {
+    const int c = task % W, q = task / W;
+    if (row_frac == 0) {
+#pragma unroll
+      for (int j = 0; j < 4; j++) tmp[(4 * q + j) * W + c] = (short)((int)interT[c * L::THP + 4 * q + j + 3] - bias);
+      continue;
+    }
+    const uint32_t *wp = (const uint32_t *)(interT + c * L::THP) + 2 * q;
+    const uint32_t w[6] = {wp[0], wp[1], wp[2], wp[3], wp[4], wp[5]};
+    int s[4];
+    filt4_words16<true>(w, yt, s);
+#pragma unroll
+    for (int j = 0; j < 4; j++) tmp[(4 * q + j) * W + c] = (short)(rshift_round(s[j], 7) - bias);
+  }
+}
+
+// mc_avg (mc.rs:454-479) of two packed i16 preps into W x H pixels
+template <typename T, int W, int H>
+__device__ __forceinline__ void mc_avg_warp(const short *t0, const short *t1, T *pred, int bit_depth, int lane) {
+  const int ib = 4 - (bit_depth == 12 ? 2 : 0);
+  const int maxv = (1 << bit_depth) - 1;
+  const int bias2 = bit_depth == 8 ? 0 : 2 * 8192;
+  for (int i = lane; i < W * H; i += 32)
+    pred[i] = (T)min(max(rshift_round((int)t0[i] + (int)t1[i] + bias2, ib + 1), 0), maxv);
 }
 
 }  // namespace
