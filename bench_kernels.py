@@ -425,6 +425,106 @@ def inter_screen(ctx):
             ctx.plane_free(p)
 
 
+def cdef_rdo(ctx):
+    """b200_cdef_rdo_dev over whole 1080p 4:2:0 frames: 8 and 10 bit, cdef_bits 0 and 3, areas of 1x1 and 2x2
+    superblocks (trimmed at the frame's edge), 30 % of the 8x8 blocks skipped, the winner's pixels written.  The
+    fused results are checked against the CPU oracle on the same frame.  Beside it, what a caller can launch
+    today: b200_cdef_find_dir_dev once, then per index the CDEF filter for three planes, b200_cdef_dist_dev over
+    the luma 8x8 blocks and b200_weighted_sse_dev over the chroma blocks.  That chain takes no decision, filters
+    with frame-relative edges (so its output is not the reference's) and has no cost or argmin: a lower bound."""
+    from tests.test_oracle_cdef_rdo import DEFAULT_STRENGTHS, cdef_rdo as orc_cdef_rdo, make_frame
+    rng = np.random.default_rng(31)
+    W, H, PAD = 1920, 1080, 8
+    sbw, sbh = 30, 17
+    w8, h8 = W // 8, (H + 7) // 8
+    for bd in (8, 10):
+        rec, src = make_frame(rng, W, H, "420", bd)
+        skip8 = (rng.random((h8, w8)) < 0.3).astype(np.uint8)
+        bpp = rec[0].itemsize
+        d_rec = [ctx.plane_from_host(r, PAD) for r in rec]
+        d_src = [ctx.plane_from_host(s, PAD) for s in src]
+        d_out = [ctx.plane_from_host(r, PAD) for r in rec]
+        d_skip = dev(skip8)
+        for cdef_bits in (0, 3):
+            n_idx = 1 << cdef_bits
+            for a in (1, 2):
+                areas = [(x, y, min(a, sbw - x), min(a, sbh - y)) for y in range(0, sbh, a) for x in range(0, sbw, a)]
+                n = len(areas)
+                d_err = torch.empty(n * 16 * 8 * 8, dtype=torch.uint8, device="cuda")
+                d_cost = torch.empty(n * 16 * 8 * 8, dtype=torch.uint8, device="cuda")
+                d_best = torch.empty(n * 16, dtype=torch.uint8, device="cuda")
+                ys, us = DEFAULT_STRENGTHS, DEFAULT_STRENGTHS[::-1]
+
+                def fused():
+                    ctx.cdef_rdo_dev(d_rec, d_src, d_out, 1, 1, W, H, bd, 5, cdef_bits, ys, us, d_skip, None,
+                                     (16384, 16384, 16384), 1000.0, areas, None, d_err, d_cost, d_best)
+                ms = timed(fused, reps=10)
+                want_out = [r.copy() for r in rec]
+                err, cost, best = orc_cdef_rdo(rec, src, want_out, 1, 1, W, H, bd, 5, cdef_bits, ys, us, skip8, None,
+                                               (16384,) * 3, 1000.0, areas)
+                got_best = d_best.cpu().numpy().view(np.int8)
+                got_err = d_err.cpu().numpy().view(np.uint64).reshape(n * 16, 8)
+                inside = np.zeros(n * 16, bool)      # slots of superblocks inside their area; the rest are not written
+                for k, (_, _, aw, ah) in enumerate(areas):
+                    for y in range(ah):
+                        inside[k * 16 + y * 4:k * 16 + y * 4 + aw] = True
+                dec = inside & (best[:n * 16] >= 0)
+                same = bool((got_best[inside] == best[:n * 16][inside]).all()
+                            and (got_err[dec, :n_idx] == err[:n * 16][dec, :n_idx]).all())
+                for p in range(3):
+                    got = np.empty_like(rec[p])
+                    ctx.check(ctx.L.b200_plane_download(ctx.h, C.byref(d_out[p]), got.ctypes.data, got.strides[0]))
+                    same = same and bool((got == want_out[p]).all())
+                assert same, f"{bd}-bit cdef_bits {cdef_bits} {a}x{a}: b200_cdef_rdo_dev disagrees with the oracle"
+                nsb = sbw * sbh
+                tile = (68 * 68 + 2 * 36 * 36) * bpp
+                nbytes = tile + 2 * (64 * 64 + 2 * 32 * 32) * bpp + 64 + n_idx * 16 + 1
+                emit(f"cdef_rdo_dev {bd}-bit cdef_bits {cdef_bits} {a}x{a} areas (filter + dist + cost + argmin, fused)",
+                     nsb, "superblocks", ms, nbytes,
+                     "1080p 4:2:0, 30 % skipped 8x8 blocks, winner written; bytes per superblock: rec tiles with halo "
+                     "+ src + out + skip flags + err/cost/best",
+                     extra={"bit_depth": bd, "cdef_bits": cdef_bits, "area_sb": a, "areas": n, "ms_per_frame": ms,
+                            "same_as_oracle": same})
+                if a == 2:
+                    continue
+                # the unfused chain: the same work through the existing launches, frame-relative edges
+                d_dir = torch.empty(w8 * h8, dtype=torch.uint8, device="cuda")
+                d_var = torch.empty(w8 * h8 * 4, dtype=torch.uint8, device="cuda")
+                tmp = [ctx.plane_from_host(r, PAD) for r in rec]
+                lb = np.zeros(w8 * h8, B.BLOCK_DTYPE)
+                lb["x"], lb["y"] = np.tile(np.arange(w8) * 8, h8), np.repeat(np.arange(h8) * 8, w8)
+                cb = lb.copy()
+                cb["x"] //= 2
+                cb["y"] //= 2
+                d_lb, d_cb = dev(lb), dev(cb)
+                d_scale = dev(np.full((h8 * 2) * (w8 * 2), 16384, np.uint32))
+                d_dist = torch.empty(w8 * h8 * 8, dtype=torch.uint8, device="cuda")
+                strengths = [dev(np.full(sbw * sbh, v, np.uint8)) for v in ys + us]
+                h8p = (H + 7) & ~7
+
+                def unfused():
+                    ctx.cdef_find_dir_dev(d_rec[0], bd, d_skip, d_dir, d_var)
+                    for i in range(n_idx):
+                        for p in range(3):
+                            ctx.cdef_filter_plane_dev(d_rec[p], tmp[p], p, int(p > 0), int(p > 0), W, h8p, bd, 5, d_skip,
+                                                      d_dir, d_var, strengths[i if p == 0 else 8 + i])
+                        ctx.cdef_dist_dev(d_src[0], tmp[0], d_lb, w8 * h8, 8, 8, bd, d_dist)
+                        for p in (1, 2):
+                            ctx.weighted_sse_dev(d_src[p], tmp[p], d_cb, w8 * h8, 4, 4, d_scale, w8 * 2, d_dist)
+                ms2 = timed(unfused, reps=10)
+                emit(f"cdef find_dir + (filter x3 + cdef_dist + weighted_sse x2) per index, {bd}-bit cdef_bits "
+                     f"{cdef_bits} (lower bound of the unfused composition)", nsb, "superblocks", ms2,
+                     nbytes + n_idx * (2 * (64 * 64 + 2 * 32 * 32) * bpp * 2),
+                     "frame-relative edges, so its output is NOT the reference's area-relative one; no cost, argmin "
+                     "or winner write: a lower bound for today's composition",
+                     extra={"bit_depth": bd, "cdef_bits": cdef_bits, "ms_per_frame": ms2,
+                            "fused_1x1_speedup": ms2 / ms})
+                for p in tmp:
+                    ctx.plane_free(p)
+        for p in d_rec + d_src + d_out:
+            ctx.plane_free(p)
+
+
 def main():
     torch.cuda.set_device(0)
     stream = torch.cuda.Stream()
@@ -439,6 +539,9 @@ def main():
         return
     if "--inter-screen" in sys.argv[1:]:
         inter_screen(ctx)
+        return
+    if "--cdef-rdo" in sys.argv[1:]:
+        cdef_rdo(ctx)
         return
     rng = np.random.default_rng(0)
     W, H, PAD = 1920, 1080, 96

@@ -693,6 +693,45 @@ int b200_cdef_tiles_dev(b200_ctx *ctx, const b200_cdef_item *items, size_t nitem
                         int luma_width, int luma_height, int bit_depth, int damping, const uint8_t *d_strength_sb,
                         int find_dir, int filter);
 
+/* The CDEF pass of rdo_loop_decision (rdo.rs:2104-2567; the RestorationFilter::None and no-LRU branches,
+ * i.e. the whole first pass and every pass when restoration is off) for many loop-restoration areas in one
+ * asynchronous call on the context's stream, without host synchronisation.  Per area the reference takes a
+ * scratch copy of the area cropped to the visible frame and rounded up to 8 (rdo.rs:2152-2157, 2277-2284),
+ * so CDEF's edge flags treat everything outside the AREA as unavailable, even where the frame continues.
+ * For each superblock of an area that has a coded 8x8 block (rdo.rs:2185-2205) and each cdef index
+ * 0 .. 1 << cdef_bits: cdef_filter_superblock with that index's strengths (skipped 8x8 blocks copied), then
+ * rdo_loop_plane_error per plane (luma cdef_dist_kernel 8x8 times the 8x8 block's frame-absolute
+ * distortion_scale; chroma sse_wxh with that bias per 4x4 chunk; the plane's sum times dist_scale[p]),
+ * summed over planes; then compute_rd_cost (an fma in f64) with the slot's rate; the first minimum wins.
+ *
+ * rec / src / out: HOST arrays of `planes` (1 = 4:0:0, or 3) frame planes: the deblocked reconstruction,
+ * the input, and (out may be NULL) the area's CDEF output after the pass, written over each area's scratch
+ * rect only: the winner's filter output for decided superblocks, a copy of rec for CDEF-skipped ones.
+ * Planes cover at least the frame rounded up to 8 luma pixels; out must not alias rec.
+ * frame_width / frame_height = fi.width / fi.height.  d_skip8: one byte per 8x8 luma block of the frame
+ * (AND of its four 4x4 skips), ceil(W/8) per row, as b200_cdef_find_dir_dev; NULL = none skipped.
+ * d_imp_scales: the Q14 distortion scale per 8x8 importance block (b200_distortion_scales_dev's ceil
+ * grid); NULL = the default scale (no temporal RDO).  dist_scale = fi.dist_scale (Q14, host).
+ * areas: HOST array; slot area * 16 + sby * 4 + sbx addresses a superblock inside its area.
+ * d_rate: one rate (1/8 bit) per slot, NULL = 0.  Outputs per slot: d_err[slot * 8 + i] (ScaledDistortion
+ * summed over planes) and d_cost[slot * 8 + i] for i < 1 << cdef_bits, written for decided superblocks
+ * only; d_best[slot] = the winning index, or -1 for a CDEF-skipped superblock.  Slots outside an area are
+ * not written.  Rejected with B200_ERR_ARG before any launch: NULL pointers, a bpp that does not match
+ * bit_depth (8 / 10 / 12), planes other than 1 / 3, a chroma layout other than 4:2:0 / 4:2:2 / 4:4:4,
+ * cdef_bits outside 0..3, a used strength above 63, damping outside 3..6 (fi.cdef_damping =
+ * 3 + (base_q_idx >> 6)), planes smaller than the frame, areas outside the frame, larger than 4x4
+ * superblocks or overlapping each other, out aliasing rec.  n_areas == 0 launches nothing. */
+typedef struct {
+  int32_t sbx, sby;   /* frame-absolute superblock of the area's top-left (tile sbo + base_sbo) */
+  int32_t sb_w, sb_h; /* 1..4 each, already trimmed to the tile as rdo.rs:2146-2147 does */
+} b200_cdef_rdo_area;
+int b200_cdef_rdo_dev(b200_ctx *ctx, const b200_plane *rec, const b200_plane *src, const b200_plane *out, int planes,
+                      int xdec, int ydec, int frame_width, int frame_height, int bit_depth, int damping, int cdef_bits,
+                      const uint8_t y_strengths[8], const uint8_t uv_strengths[8], const uint8_t *d_skip8,
+                      const uint32_t *d_imp_scales, const uint32_t dist_scale[3], double lambda,
+                      const b200_cdef_rdo_area *areas, size_t n_areas, const uint32_t *d_rate, uint64_t *d_err,
+                      double *d_cost, int8_t *d_best);
+
 /* ------------------------------------------------------- intra prediction (predict.rs)
  * Boundary = rust::dispatch_predict_intra(mode, variant, dst, tx_size, bit_depth, ac, angle,
  * ief_params, edge_buf, cpu) (predict.rs:705-784; the asm wrappers, asm/x86/predict.rs:239-873,

@@ -46,6 +46,11 @@ class CdefItem(C.Structure):
                 ("rw8", C.c_int32), ("rh8", C.c_int32)]
 
 
+class CdefRdoArea(C.Structure):
+    """b200_cdef_rdo_area: a loop-restoration area in frame-absolute superblocks."""
+    _fields_ = [("sbx", C.c_int32), ("sby", C.c_int32), ("sb_w", C.c_int32), ("sb_h", C.c_int32)]
+
+
 class FramePipeCfg(C.Structure):
     _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("pad", C.c_int32), ("bpp", C.c_int32),
                 ("bit_depth", C.c_int32), ("block_w", C.c_int32), ("block_h", C.c_int32), ("lambda_", C.c_uint32),
@@ -241,6 +246,7 @@ def lib():
     L.b200_pred_cfl_ac_dev.argtypes = [vp, pp, vp, sz] + [i32] * 6 + [vp]
     L.b200_intra_mode_screen_dev.argtypes = [vp, pp, pp] + [i32] * 6 + [vp, sz, vp, vp]
     L.b200_inter_mode_screen_dev.argtypes = [vp, pp] + [i32] * 4 + [vp] + [i32] * 5 + [vp, sz, vp, vp]
+    L.b200_cdef_rdo_dev.argtypes = [vp, vp, vp, vp] + [i32] * 8 + [vp] * 5 + [C.c_double, vp, sz, vp, vp, vp, vp]
     _LIB = L
     return L
 
@@ -499,6 +505,28 @@ class Context:
         self.check(self.L.b200_cdef_tiles_dev(self.h, C.addressof(items), len(items), plane, xdec, ydec, luma_w,
                                               luma_h, bit_depth, damping, _dev_ptr(d_strength_sb), int(find_dir),
                                               int(filter)))
+
+    def cdef_rdo_dev(self, rec, src, out, xdec, ydec, width, height, bit_depth, damping, cdef_bits, y_strengths,
+                     uv_strengths, d_skip8, d_imp_scales, dist_scale, lam, areas, d_rate, d_err, d_cost, d_best):
+        """rec / src / out: lists of 1 or 3 Plane (out may be None); areas: [(sbx, sby, sb_w, sb_h), ...];
+        d_err (n_areas * 16 * 8 u64), d_cost (same, f64), d_best (n_areas * 16 i8) (include/b200rdo.h)."""
+        def arr(planes):
+            if planes is None:
+                return None
+            a = (Plane * len(planes))()
+            for k, p in enumerate(planes):
+                C.memmove(C.byref(a[k]), C.byref(p), C.sizeof(Plane))
+            return a
+        r, s_, o = arr(rec), arr(src), arr(out)
+        ar = np.ascontiguousarray(np.asarray(areas, np.int32).reshape(-1, 4))   # b200_cdef_rdo_area rows
+        ys = (C.c_uint8 * 8)(*[int(v) for v in y_strengths])
+        us = (C.c_uint8 * 8)(*[int(v) for v in uv_strengths])
+        ds = (C.c_uint32 * 3)(*[int(v) for v in dist_scale])
+        self.check(self.L.b200_cdef_rdo_dev(
+            self.h, C.addressof(r), C.addressof(s_), C.addressof(o) if o is not None else None, len(rec), xdec, ydec,
+            width, height, bit_depth, damping, cdef_bits, C.addressof(ys), C.addressof(us), _dev_ptr(d_skip8),
+            _dev_ptr(d_imp_scales), C.addressof(ds), float(lam), ar.ctypes.data, len(areas), _dev_ptr(d_rate),
+            _dev_ptr(d_err), _dev_ptr(d_cost), _dev_ptr(d_best)))
 
     # ---- intra prediction
     def predict_intra_dev(self, d_edges, d_items, n, d_ac, w, h, bit_depth, plane_w, plane_h, d_out):

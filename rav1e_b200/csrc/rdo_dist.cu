@@ -15,11 +15,9 @@
 #include <algorithm>
 #include <mutex>
 
-#include "common.cuh"
+#include "rdo_dist_dev.cuh"
 
 namespace {
-
-constexpr int kWsseShift = 8;  // GET_WEIGHTED_SSE_SHIFT, dist.rs:223
 
 // dist.rs:234-283.  scale: one Q14 DistortionScale per 4x4 chunk of the plane (chunk (cx, cy)
 // at scale[cy * scale_stride + cx]); blocks sit on 4-pixel positions.
@@ -47,42 +45,12 @@ __global__ void __launch_bounds__(256) weighted_sse_kernel(PlaneView a, PlaneVie
           sum += (uint32_t)(d * d);
         }
       }
-      const unsigned long long s = scale[(long long)((blk.y >> 2) + cy) * scale_stride + (blk.x >> 2) + cx];
-      acc += ((unsigned long long)sum * s + ((1u << kWsseShift) >> 1)) >> kWsseShift;
+      acc += wsse_chunk(sum, scale[(long long)((blk.y >> 2) + cy) * scale_stride + (blk.x >> 2) + cx]);
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-    if (lane == 0) {
-      // den = DistortionScale::new(1, 1 << 8).0 = ((1 << 14) + 128) / 256 = 64 (rdo.rs:579-583)
-      constexpr unsigned long long den = ((1ull << 14) + ((1u << kWsseShift) / 2)) >> kWsseShift;
-      out[i] = (acc + (den >> 1)) / den;
-    }
+    if (lane == 0) out[i] = wsse_finish(acc);
   }
-}
-
-// round(2^14 / (1 + x)), dist.rs:288-297
-__constant__ unsigned short kAreaDivisors[64] = {
-    16384, 8192, 5461, 4096, 3277, 2731, 2341, 2048, 1820, 1638, 1489, 1365, 1260, 1170, 1092, 1024,
-    964,   910,  862,  819,  780,  745,  712,  683,  655,  630,  607,  585,  565,  546,  529,  512,
-    496,   482,  468,  455,  443,  431,  420,  410,  400,  390,  381,  372,  364,  356,  349,  341,
-    334,   328,  321,  315,  309,  303,  298,  293,  287,  282,  278,  273,  269,  264,  260,  256};
-
-// activity.rs:159-186 with ssim_boost_rsqrt :107-143 inlined
-__device__ __forceinline__ uint32_t apply_ssim_boost(uint32_t input, uint32_t svar, uint32_t dvar, int bit_depth) {
-  const int coeff_shift = bit_depth - 8;
-  const unsigned long long sv = svar >> (2 * coeff_shift), dv = dvar >> (2 * coeff_shift);
-  constexpr unsigned long long C1 = 3355, C2 = 16128, C3 = 12338;
-  constexpr int RATIO_SHIFT = 14;
-  constexpr unsigned long long RATIO = (((C1 << (RATIO_SHIFT + 1)) / C3) + 1) >> 1;
-  const unsigned long long x = C1 * C1 + sv * dv;
-  const int k = (63 - __clzll((long long)x)) >> 1;
-  const int s = 2 * k - (16 - 2);
-  const uint32_t t = (uint32_t)(s > 0 ? x >> s : x << -s) & 0xffffu;  // `as u16`
-  const int shift = 14 + ((s + 16) >> 1);
-  const int nn = (int)t - 32768;
-  const int inner = -13490 + ((nn * 6711) >> 15);
-  const uint32_t norm = (uint32_t)(23557 + ((nn * inner) >> 15)) & 0xffffu;
-  return (uint32_t)(((unsigned long long)input * (((RATIO * (sv + dv + C2)) * (unsigned long long)norm) >> RATIO_SHIFT)) >> shift);
 }
 
 // dist.rs:302-372
@@ -105,14 +73,8 @@ __global__ void __launch_bounds__(128) cdef_dist_kernel(PlaneView src, PlaneView
         sum_sd += s * d;
       }
     }
-    const uint32_t sse = sum_d2 + sum_s2 - 2 * sum_sd;
-    const unsigned long long S = sum_s, D = sum_d, div = kAreaDivisors[w * h - 1];
-    const uint32_t ms = (uint32_t)((S * S * div + (1u << 13)) >> 14);
-    const uint32_t md = (uint32_t)((D * D * div + (1u << 13)) >> 14);
-    uint32_t svar = sum_s2 > ms ? sum_s2 - ms : 0u;  // saturating_sub
-    uint32_t dvar = sum_d2 > md ? sum_d2 - md : 0u;
-    svar = (uint32_t)(((unsigned long long)svar * div + (1u << 7)) >> 8);  // scale to an 8x8 area
-    dvar = (uint32_t)(((unsigned long long)dvar * div + (1u << 7)) >> 8);
+    uint32_t svar, dvar;
+    const uint32_t sse = cdef_dist_vars(sum_s, sum_d, sum_s2, sum_d2, sum_sd, w * h, &svar, &dvar);
     if (raw) {  // what the asm kernels return (asm/x86/dist/cdef_dist.rs:18-24)
       raw[3 * i + 0] = svar;
       raw[3 * i + 1] = dvar;
