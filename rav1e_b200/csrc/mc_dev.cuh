@@ -6,7 +6,9 @@
 // inter = px << ib exactly (128 px is a multiple of 2^(7-ib)), after which the V rounding
 // (sum + 2^(6+ib)) >> (7+ib) equals the V-only (sum + 64) >> 7; an identity V pass turns
 // round(128 * inter, 7+ib) into round(inter, ib), the H-only case's second rounding; and the i16
-// intermediate never truncates (|inter| <= 20.5 K at every bit depth).  So one code path serves all.
+// intermediate never truncates.  Its extremes, every positive tap on max or every negative one, are
+// SHARP's half-pel row (taps summing to +184 and -56): inter lies in [-1 785, 5 865] at 8 bit,
+// [-7 161, 23 529] at 10 bit and [-7 166, 23 546] at 12 bit.  So one code path serves all.
 //   prep_8tap  src/mc.rs:360-451 (the compound path's i16 predictions, PREP_BIAS 8192 subtracted at 10/12 bit)
 // has the same four cases with one rounding less: integer copy px << ib, V only round_shift(sum, 7-ib),
 // H only round_shift(sum, 7-ib), HV round_shift(sum, 7) over the same i16 intermediate.  The identity

@@ -172,10 +172,11 @@ class ViewPlane:
         self.plane.alloc = base if with_alloc else None
 
 
-def profiled_kernels(fn):
-    """Run `fn` under torch.profiler and return the motion-estimation kernels it launched, in
-    launch order, as `name<template args>` (e.g. `me_cand_group_u8<16, 16, false>`).  Fails when
-    the profiler saw no device activity at all: an empty list must mean "no ME kernel ran"."""
+def profiled_kernels(fn, prefix="me_"):
+    """Run `fn` under torch.profiler and return the kernels whose names start with `prefix` (by
+    default the motion-estimation kernels) in launch order, as `name<template args>` (e.g.
+    `me_cand_group_u8<16, 16, false>`).  Fails when the profiler saw no device activity at all: an
+    empty list must mean "no such kernel ran"."""
     import re
     import time
     import torch
@@ -195,7 +196,7 @@ def profiled_kernels(fn):
     assert dev, "torch.profiler recorded no CUDA kernels on this machine: kernel routing cannot be checked"
     names = []
     for n in dev:
-        m = re.search(r"\b(me_\w+(?:<[^()]*>)?)\(", n)
+        m = re.search(r"\b(" + prefix + r"\w+(?:<[^()]*>)?)\(", n)
         if m:
             names.append(m.group(1))
     return names

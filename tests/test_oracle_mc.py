@@ -164,3 +164,101 @@ def test_put_equals_the_specification_two_pass_form(dtype, bd):
                     want[r, c] = min(max(rnd(int((ky * inter[r:r + 8, c]).sum()), r1), 0), maxv)
             got = O.put_8tap(p, x0, y0, w, h, cf, rf, mx, my, bd)
             np.testing.assert_array_equal(got, want, err_msg=f"{w}x{h} frac ({cf},{rf}) modes ({mx},{my})")
+
+
+@pytest.mark.parametrize("bd", [8, 10, 12])
+def test_intermediate_extremes_fit_i16(bd):
+    """The kernels keep the horizontal pass in an i16 intermediate and run every sub-pel case through it
+    (mc_dev.cuh).  That rests on the intermediate never truncating: its extremes, every positive tap on max or
+    every negative tap on max, over every bank, fraction and length, lie inside i16.  The vertical pass of
+    `prep` over those extremes, the value stored as i16, fits too."""
+    L = O.lib()
+    f = (C.c_int32 * 8)()
+    r0 = 5 if bd == 12 else 3
+    maxv = (1 << bd) - 1
+    rnd = lambda v, b: (v + (1 << (b - 1))) >> b
+    rows = []
+    for mode in range(4):
+        for length in (4, 8):
+            for frac in range(16):
+                L.orc_get_filter(mode, frac, length, f)
+                rows.append(list(f))
+    hi = max(rnd(sum(t for t in r if t > 0) * maxv, r0) for r in rows)
+    lo = min(rnd(sum(t for t in r if t < 0) * maxv, r0) for r in rows)
+    assert -32768 <= lo and hi <= 32767
+    assert (hi, lo) == {8: (5865, -1785), 10: (23529, -7161), 12: (23546, -7166)}[bd]
+    bias = 0 if bd == 8 else 8192
+    for r in rows:
+        top = sum(t * (hi if t > 0 else lo) for t in r)
+        bottom = sum(t * (lo if t > 0 else hi) for t in r)
+        assert -32768 <= rnd(bottom, 7) - bias and rnd(top, 7) - bias <= 32767
+
+
+@pytest.mark.parametrize("dtype,bd", [(np.uint8, 8), (np.uint16, 10), (np.uint16, 12)])
+def test_numpy_reference_of_the_gpu_sweeps_equals_the_oracle(dtype, bd):
+    """tests/test_mc_paths_gpu.py compares the kernels with a vectorised restatement of the specification's
+    two-pass form; on one random batch per bit depth it must equal orc_mc_blocks and orc_mc_avg."""
+    from tests import test_mc_paths_gpu as T
+    rng = np.random.default_rng(7 + bd)
+    p = make_plane(dtype, bd, seed=bd, w=96, h=80, pad=24)
+    full = p.data.astype(np.int64)
+    for (w, h), (xdec, ydec), (mx, my) in (((8, 8), (0, 0), (2, 1)), ((4, 16), (1, 0), (0, 3)),
+                                           ((16, 4), (1, 1), (1, 2)), ((2, 2), (1, 1), (3, 0))):
+        blocks, mvs = T.random_items(rng, 40, w, h, xdec, ydec, 96, 80, 8)
+        x0, y0, cf, rf = T.mv_params(blocks, mvs, xdec, ydec)
+        T.assert_readable(x0, y0, w, h, 96, 80, 24)
+        for kind in (0, 1):
+            want = O.mc_blocks(p, blocks, mvs, w, h, mx, my, bd, xdec, ydec, kind)
+            got = T.mc_ref(full, 24, x0, y0, cf, rf, w, h, mx, my, bd, kind)
+            np.testing.assert_array_equal(got, want, err_msg=f"{w}x{h} kind {kind}")
+        t1 = O.mc_blocks(p, blocks, mvs, w, h, mx, my, bd, xdec, ydec, 1)
+        t2 = O.mc_blocks(p, blocks, mvs[::-1].copy(), w, h, my, mx, bd, xdec, ydec, 1)
+        np.testing.assert_array_equal(T.avg_ref(t1, t2, bd), np.stack([O.mc_avg(a, b, bd) for a, b in zip(t1, t2)]))
+
+
+@pytest.mark.parametrize("dtype,bd", [(np.uint8, 8), (np.uint16, 10), (np.uint16, 12)])
+def test_prep_and_avg_equal_the_specification_at_extreme_tiles(dtype, bd):
+    """The specification's compound form (7.11.3.4 with InterRound1 = 7, then 7.11.3.15's average rounded by
+    InterPostRound) on tiles built from the tap signs, which put the intermediate at its extremes: `prep` is the
+    horizontal pass rounded by InterRound0, the vertical pass rounded by 7, minus PREP_BIAS at 10 / 12 bit, and
+    `avg` is (t1 + t2 + 2 PREP_BIAS) rounded by InterPostRound (5; 3 at 12 bit), then Clip1.  `put` is checked on
+    the same tiles."""
+    from tests.test_mc_paths_gpu import sign_tiles
+    L = O.lib()
+    r0, r1 = (5, 9) if bd == 12 else (3, 11)
+    post = 3 if bd == 12 else 5
+    bias = 0 if bd == 8 else 8192
+    maxv = (1 << bd) - 1
+    rnd = lambda v, b: (v + (1 << (b - 1))) >> b
+    fx, fy = (C.c_int32 * 8)(), (C.c_int32 * 8)()
+    w = h = 8
+    for mx, my, cf, rf in ((2, 2, 8, 8), (2, 0, 8, 6), (0, 2, 4, 8), (1, 3, 9, 5), (2, 2, 7, 0), (2, 2, 0, 9)):
+        L.orc_get_filter(mx, cf, w, fx)
+        L.orc_get_filter(my, rf, h, fy)
+        kx, ky = np.array(list(fx), np.int64), np.array(list(fy), np.int64)
+        preps = []
+        for tile in sign_tiles(kx, ky, maxv):
+            p = O.Plane(16, 16, 8, dtype=dtype)
+            p.fill_from(np.tile(tile, (2, 2)).astype(dtype))
+            img = p.data.astype(np.int64)
+            inter = np.zeros((h + 7, w), np.int64)
+            for r in range(h + 7):
+                for c in range(w):
+                    inter[r, c] = rnd(int((kx * img[p.pad + r, p.pad + c:p.pad + c + 8]).sum()), r0)
+            want_put = np.zeros((h, w), np.int64)
+            want_prep = np.zeros((h, w), np.int64)
+            for r in range(h):
+                for c in range(w):
+                    s = int((ky * inter[r:r + 8, c]).sum())
+                    want_put[r, c] = min(max(rnd(s, r1), 0), maxv)
+                    want_prep[r, c] = rnd(s, 7) - bias
+            what = f"modes ({mx},{my}) frac ({cf},{rf})"
+            np.testing.assert_array_equal(O.put_8tap(p, 3, 3, w, h, cf, rf, mx, my, bd), want_put, err_msg=what)
+            got = O.prep_8tap(p, 3, 3, w, h, cf, rf, mx, my, bd)
+            np.testing.assert_array_equal(got, want_prep, err_msg=what)
+            preps.append(got.astype(np.int64))
+        for a in range(len(preps)):
+            for b in (a, a ^ 1):
+                want = np.clip(rnd(preps[a] + preps[b] + 2 * bias, post), 0, maxv)
+                got = O.mc_avg(preps[a].astype(np.int16), preps[b].astype(np.int16), bd)
+                np.testing.assert_array_equal(got, want, err_msg=f"avg {what} tiles {a} {b}")
