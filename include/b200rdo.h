@@ -681,7 +681,15 @@ int b200_cdef_filter_rect_dev(b200_ctx *ctx, const b200_plane *in, const b200_pl
 /* Many (plane, tile) items per call - the tiles a rank owns across the frames of a batch - served by
  * as few launches as possible (32 items per launch): with find_dir the directions / variances of every
  * item's blocks are (re)computed from `in` (luma only), with filter every item's rect of `in` is
- * filtered into `out`.  `items` is a HOST array; the arrays an item points to are frame-indexed. */
+ * filtered into `out`.  `items` is a HOST array; the arrays an item points to are frame-indexed.
+ * This call and the four above check every argument and every item before the first launch, and
+ * reject with B200_ERR_ARG (nothing launched, nothing written): a luma size that is not a positive
+ * multiple of 8, a bit depth other than 8 / 10 / 12, a chroma layout other than 4:4:4 / 4:2:2 / 4:2:0,
+ * plane 0 with xdec or ydec set, find_dir on a chroma plane; with filter, damping outside 3..6
+ * (fi.cdef_damping) or NULL strengths; per item, a NULL in / dir / var, an `in` (or with filter `out`)
+ * whose bpp does not match the bit depth or that is smaller than (luma_width >> xdec) x
+ * (luma_height >> ydec) or has a stride below its width, with filter an `out` that is NULL or is `in`,
+ * and a rect outside the luma 8x8 grid.  nitems == 0 launches nothing. */
 typedef struct {
   const b200_plane *in, *out; /* out may be NULL when only the directions are wanted */
   const uint8_t *d_skip8;     /* may be NULL */

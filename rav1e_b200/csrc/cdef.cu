@@ -142,20 +142,38 @@ int check_rect(b200_ctx *ctx, int w8, int h8, int rx8, int ry8, int rw8, int rh8
   return B200_OK;
 }
 
-// items [k0, k0 + n) of a host item array -> one launch of each requested kernel
+// The filter reads (and writes) the plane's (luma >> dec) area and nothing outside it, so a smaller
+// plane would give wrong pixels without any fault: it is rejected.
+int check_plane(b200_ctx *ctx, const b200_plane *p, size_t k, const char *what, int width, int height, int bpp) {
+  B200_REQUIRE(ctx, p->bpp == bpp, "item %zu: %s bpp %d, expected %d", k, what, p->bpp, bpp);
+  B200_REQUIRE(ctx, p->width >= width && p->height >= height && p->stride >= p->width,
+               "item %zu: %s plane %dx%d (stride %d) smaller than the %dx%d the filter covers", k, what, p->width,
+               p->height, p->stride, width, height);
+  return B200_OK;
+}
+
+int check_item(b200_ctx *ctx, const b200_cdef_item &q, size_t k, int xdec, int ydec, int luma_width, int luma_height,
+               int bit_depth, int do_filter) {
+  B200_REQUIRE(ctx, q.in && q.in->data && q.d_dir && q.d_var, "item %zu: NULL plane / dir / var", k);
+  const int bpp = bit_depth == 8 ? 1 : 2;
+  if (int st = check_plane(ctx, q.in, k, "in", luma_width >> xdec, luma_height >> ydec, bpp)) return st;
+  if (do_filter) {
+    B200_REQUIRE(ctx, q.out && q.out->data && q.out->data != q.in->data,
+                 "item %zu: the filter needs a distinct output plane (taps read unfiltered neighbours)", k);
+    if (int st = check_plane(ctx, q.out, k, "out", luma_width >> xdec, luma_height >> ydec, bpp)) return st;
+  }
+  return check_rect(ctx, luma_width >> 3, luma_height >> 3, q.rx8, q.ry8, q.rw8, q.rh8);
+}
+
+// items [k0, k0 + n) of a host item array, already checked -> one launch of each requested kernel
 int cdef_launch(b200_ctx *ctx, const b200_cdef_item *items, int n, int plane, int xdec, int ydec, int luma_width,
                 int luma_height, int bit_depth, int damping, const uint8_t *d_strength_sb, int do_dir, int do_filter) {
   CdefItems it{};
   it.n = n;
-  int max_w8 = 0, max_h8 = 0, bpp = 0;
+  int max_w8 = 0, max_h8 = 0;
+  const int bpp = bit_depth == 8 ? 1 : 2;
   for (int k = 0; k < n; k++) {
     const b200_cdef_item &q = items[k];
-    B200_REQUIRE(ctx, q.in && q.in->data && q.d_dir && q.d_var, "item %d: NULL plane / dir / var", k);
-    B200_REQUIRE(ctx, !do_filter || (q.out && q.out->data && q.out->data != q.in->data && q.out->bpp == q.in->bpp),
-                 "item %d: the filter needs a distinct output plane (taps read unfiltered neighbours)", k);
-    B200_REQUIRE(ctx, (q.in->bpp == 1) == (bit_depth == 8), "bpp %d vs bit depth %d", q.in->bpp, bit_depth);
-    if (int st = check_rect(ctx, luma_width >> 3, luma_height >> 3, q.rx8, q.ry8, q.rw8, q.rh8)) return st;
-    bpp = q.in->bpp;
     it.in[k] = q.in->data;
     it.in_stride[k] = q.in->stride;
     it.out[k] = do_filter ? q.out->data : nullptr;
@@ -168,7 +186,6 @@ int cdef_launch(b200_ctx *ctx, const b200_cdef_item *items, int n, int plane, in
     max_h8 = std::max(max_h8, q.rh8);
   }
   if (do_dir) {
-    B200_REQUIRE(ctx, plane == 0 && xdec == 0 && ydec == 0, "directions are searched on the luma plane");
     const dim3 grid(std::max(1, std::min((max_w8 * max_h8 + 127) / 128, ctx->num_sms * 16 / n)), n);
     if (bpp == 1)
       cdef_find_dir_kernel<uint8_t><<<grid, 128, 0, ctx->stream>>>(it, luma_width >> 3, bit_depth - 8);
@@ -177,7 +194,6 @@ int cdef_launch(b200_ctx *ctx, const b200_cdef_item *items, int n, int plane, in
     B200_LAUNCH_CHECK(ctx);
   }
   if (do_filter) {
-    B200_REQUIRE(ctx, d_strength_sb, "NULL strengths");
     CdefPlaneArgs a;
     a.plane = plane;
     a.xdec = xdec;
@@ -204,10 +220,22 @@ int cdef_items(b200_ctx *ctx, const b200_cdef_item *items, size_t nitems, int pl
   B200_REQUIRE(ctx, ctx != nullptr, "ctx is NULL");
   B200_REQUIRE(ctx, (luma_width & 7) == 0 && (luma_height & 7) == 0 && luma_width > 0 && luma_height > 0,
                "luma %dx%d must be a multiple of 8 (rav1e pads frames to 8)", luma_width, luma_height);
-  B200_REQUIRE(ctx, (xdec == 0 || xdec == 1) && (ydec == 0 || ydec == 1) && plane >= 0 && plane < 3, "bad plane");
+  B200_REQUIRE(ctx, plane >= 0 && plane < 3, "bad plane %d", plane);
+  B200_REQUIRE(ctx, (xdec == 0 && ydec == 0) || (xdec == 1 && ydec == 0) || (xdec == 1 && ydec == 1),
+               "chroma layout (xdec %d, ydec %d) is not 4:4:4, 4:2:2 or 4:2:0", xdec, ydec);
+  B200_REQUIRE(ctx, plane != 0 || (xdec == 0 && ydec == 0), "luma with xdec %d, ydec %d", xdec, ydec);
+  B200_REQUIRE(ctx, !do_dir || plane == 0, "directions are searched on the luma plane");
   B200_REQUIRE(ctx, bit_depth == 8 || bit_depth == 10 || bit_depth == 12, "bad bit depth %d", bit_depth);
+  if (do_filter) {
+    // fi.cdef_damping = 3 + (base_q_idx >> 6) (encoder.rs:1221); the direction-only calls pass none
+    B200_REQUIRE(ctx, damping >= 3 && damping <= 6, "damping %d outside 3..6", damping);
+    B200_REQUIRE(ctx, d_strength_sb, "NULL strengths");
+  }
   if (nitems == 0) return B200_OK;
   B200_REQUIRE(ctx, items != nullptr, "NULL items");
+  // every item of every phase is checked before the first launch: a rejected call launches nothing
+  for (size_t k = 0; k < nitems; k++)
+    if (int st = check_item(ctx, items[k], k, xdec, ydec, luma_width, luma_height, bit_depth, do_filter)) return st;
   B200_CUDA(ctx, cudaSetDevice(ctx->device));
   // all the directions first: a tile's filter reads only its own blocks' directions, but keeping the
   // two phases apart lets one call serve callers that filter several planes from one analysis

@@ -185,7 +185,8 @@ __device__ __forceinline__ CdefBlockTaps cdef_block_taps(const uint8_t *strength
 // sentinel is stored as int16 0x8000 = -32768, so `max` ignores it on its own (every real pixel is
 // >= 0) and `min` runs on the value reinterpreted as unsigned (0xffff8000: larger than any pixel);
 // its difference to the centre is so large that constrain() returns 0 for it, exactly like the
-// reference's 0x8000 does.
+// reference's 0x8000 does.  That holds up to a final damping of 13 at 12 bit and 14 at 8 / 10 bit
+// (tests/test_oracle_cdef.py derives it); the largest the drivers pass is 6 + coeff_shift.
 __device__ __forceinline__ int cdef_filter_tile_px(const short *c, const CdefBlockTaps &b) {
   const int xv = c[0];
   int sum = 0, mx = xv;

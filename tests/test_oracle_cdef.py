@@ -71,6 +71,58 @@ def test_filter_fixed_points_and_sentinel(dtype, bd):
             assert dst.max() <= img.max() and dst.min() >= img.min()
 
 
+def np_constrain(diff, threshold, damping):
+    """constrain() of AV1 7.15.3 over an int64 array of differences (threshold > 0)."""
+    shift = max(0, damping - (int(threshold).bit_length() - 1))
+    mag = np.abs(diff)
+    v = np.clip(threshold - (mag >> shift), 0, mag)
+    return np.where(diff < 0, -v, v)
+
+
+def driver_thresholds(bd):
+    """Every nonzero pri / sec threshold the frame drivers can hand constrain(): luma's adjust_strength of
+    pri << cs in each variance bracket (var 0, then msb(var >> 6) = 0 .. 12 and beyond), chroma's pri << cs,
+    and sec << cs with sec in {1, 2, 4} (3 -> 4)."""
+    L = O.lib()
+    cs = bd - 8
+    vars_ = [0] + [64 << i for i in range(14)]
+    thr = {L.orc_cdef_adjust_strength(p << cs, v) for p in range(16) for v in vars_}
+    thr |= {p << cs for p in range(16)} | {s << cs for s in (1, 2, 4)}
+    return sorted(t for t in thr if t)
+
+
+@pytest.mark.parametrize("bd", [8, 10, 12])
+def test_sentinel_never_contributes_at_any_legal_damping(bd):
+    """cdef_dev.cuh stores CDEF_VERY_LARGE as int16 -32768 where the reference stores u16 0x8000: for every
+    threshold the drivers produce and every final damping they pass (luma 3..6 + cs, chroma one less), the
+    sentinel's constrain() term is 0 in both encodings, it never wins `max`, and as unsigned it never wins
+    `min`.  The damping at which the term first becomes nonzero is derived, and must lie above the legal range."""
+    from tests.test_oracle_cdef_spec import spec_constrain
+    cs = bd - 8
+    maxv = (1 << bd) - 1
+    x = np.arange(maxv + 1, dtype=np.int64)
+    diffs = {"u16 0x8000": 0x8000 - x, "int16 -32768": -32768 - x}
+    thresholds = driver_thresholds(bd)
+    assert max(thresholds) == 15 << cs                          # bracket 12 rounds pri 15 back to itself
+    for t in thresholds[::7]:                                   # the vector form is the specification's
+        for d in (2 + cs, 6 + cs):
+            want = [spec_constrain(int(v), t, d) for v in diffs["u16 0x8000"][::97]]
+            np.testing.assert_array_equal(np_constrain(diffs["u16 0x8000"][::97], t, d), want)
+    legal = range(2 + cs, 6 + cs + 1)
+    first_nonzero = None
+    for damping in range(2 + cs, 40):
+        hit = any(np_constrain(diff, t, damping).any() for diff in diffs.values() for t in thresholds)
+        if damping in legal:
+            assert not hit, f"sentinel contributes at legal damping {damping}"
+        if hit and first_nonzero is None:
+            first_nonzero = damping
+    assert first_nonzero is not None and first_nonzero > max(legal)
+    print(f"{bd}-bit: the sentinel term is first nonzero at final damping {first_nonzero}, legal max {max(legal)}")
+    s16 = np.int64(-32768)
+    assert (np.maximum(x, s16) == x).all()                       # max ignores the int16 sentinel
+    assert (np.minimum(x.astype(np.uint32), np.uint32(s16 & 0xFFFFFFFF)) == x).all()   # min as unsigned
+
+
 def test_frame_driver_skip_copies_and_strength_zero_is_identity():
     rng = np.random.default_rng(1)
     W, H = 128, 72

@@ -31,8 +31,8 @@ def spec_constrain(diff, threshold, damping):
     return -v if diff < 0 else v
 
 
-def spec_direction(block, bit_depth):
-    """7.15.2: returns (yDir, var)."""
+def spec_direction_costs(block, bit_depth):
+    """7.15.2: the eight direction costs."""
     cost = [0] * 8
     partial = [[0] * 15 for _ in range(8)]
     for i in range(8):
@@ -62,6 +62,12 @@ def spec_direction(block, bit_depth):
         cost[i] *= DIV_TABLE[8]
         for j in range(3):
             cost[i] += (partial[i][j] * partial[i][j] + partial[i][10 - j] * partial[i][10 - j]) * DIV_TABLE[2 * j + 2]
+    return cost
+
+
+def spec_direction(block, bit_depth):
+    """7.15.2: returns (yDir, var)."""
+    cost = spec_direction_costs(block, bit_depth)
     best, ydir = 0, 0
     for d in range(8):
         if cost[d] > best:
