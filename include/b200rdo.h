@@ -413,6 +413,9 @@ typedef struct {
   int32_t tx_size, tx_type; /* transform of the SAD winner's residual (block size = transform size); tx_size < 0: off */
   uint32_t dc_quant, ac_quant; /* ac_quant 0: raw coefficients out; else qcoeffs + eob + tx-domain distortion */
 } b200_frame_pipe_cfg;
+/* Rejects with B200_ERR_ARG: a bad geometry, bpp that does not match bit_depth, a transform that is invalid or
+ * not of the block size and, when the quantize chain is on (tx_size >= 0, ac_quant != 0), step sizes outside
+ * 1..65535 (as b200_quantize_dev), so that a bad quantizer fails here rather than in a push. */
 int b200_frame_pipe_create(b200_ctx *ctx, const b200_frame_pipe_cfg *cfg, b200_frame_pipe **out);
 void b200_frame_pipe_destroy(b200_frame_pipe *pipe);
 size_t b200_frame_pipe_nblocks(const b200_frame_pipe *pipe);
@@ -424,8 +427,9 @@ size_t b200_frame_pipe_nblocks(const b200_frame_pipe *pipe);
  * yet) and leaves the outputs untouched.
  * Copies: inputs that lie back to back in host memory in the order [frame (dense rows) | sad_offsets |
  * satd_offsets | centers] travel as ONE host->device copy, outputs laid out [best_sad | best_satd |
- * coeffs | eob | (8-byte aligned) tx_dist] as ONE device->host copy; any other layout works with a copy
- * per buffer. */
+ * coeffs | eob | (8-byte aligned) tx_dist] as ONE device->host copy (which writes zeros into the alignment
+ * gap in front of tx_dist); any other layout works with a copy per buffer, and nothing outside the
+ * buffers themselves is written. */
 int b200_frame_pipe_push(b200_frame_pipe *pipe, const void *frame, ptrdiff_t frame_stride_bytes,
                          const int8_t *sad_offsets, const int8_t *satd_offsets, const int16_t *centers,
                          b200_me_result *best_sad, b200_me_result *best_satd, void *coeffs, uint16_t *eob,
@@ -442,7 +446,8 @@ int b200_frame_pipe_set_lists(b200_frame_pipe *pipe, const int8_t *sad_offsets, 
  * distortion and - block after block in `packed` - only those eob quantized coefficients in scan order
  * (i16 for 8-bit frames, i32 for HBD).  *packed_count = total number of coefficients; when it exceeds
  * packed_capacity (in coefficients) only the first packed_capacity were copied (the call still succeeds: the
- * caller retries with a larger buffer).  best_sad / best_satd / eob / tx_dist may be NULL.  The call waits
+ * caller retries with a larger buffer).  best_sad / best_satd / eob / tx_dist may be NULL; as in a push, the
+ * winners of a leg whose list length is 0 are not written.  The call waits
  * once for the device (the size of the packed copy is a result); in asynchronous mode the packed copy itself is
  * still in flight when it returns.  The first push of a pipe only uploads: *packed_count = 0. */
 int b200_frame_pipe_push_packed(b200_frame_pipe *pipe, const void *frame, ptrdiff_t frame_stride_bytes,

@@ -162,6 +162,10 @@ extern "C" int b200_frame_pipe_create(b200_ctx *ctx, const b200_frame_pipe_cfg *
                                          b200_tx_height(cfg->tx_size) == cfg->block_h),
                "transform %d/%d does not match the %dx%d blocks", cfg->tx_size, cfg->tx_type, cfg->block_w,
                cfg->block_h);
+  // as b200_quantize_dev, here so that a bad quantizer fails before a push has enqueued anything
+  B200_REQUIRE(ctx, cfg->tx_size < 0 || cfg->ac_quant == 0 ||
+                        (cfg->dc_quant >= 1 && cfg->dc_quant <= 65535 && cfg->ac_quant <= 65535),
+               "quantizer step sizes must be NonZeroU16 (dc %u, ac %u)", cfg->dc_quant, cfg->ac_quant);
   B200_CUDA(ctx, cudaSetDevice(ctx->device));
   b200_frame_pipe *p = new b200_frame_pipe();
   p->ctx = ctx;
@@ -178,7 +182,12 @@ extern "C" int b200_frame_pipe_create(b200_ctx *ctx, const b200_frame_pipe_cfg *
     p->d_offs_sad = (uint32_t *)c.take((nb + 1) * 4);
     p->d_offs_satd = (uint32_t *)c.take((nb + 1) * 4);
     p->frame_bytes = (size_t)cfg->width * cfg->height * cfg->bpp;
-    p->d_stage = (uint8_t *)c.take(p->frame_bytes + ns * 2 + nt * 2 + nb * 4);  // dense: mirrors the host layout
+    // dense: mirrors the host layout.  It starts `lead` bytes into its carve so that the centres (read as short2)
+    // are 4-aligned whatever the frame size; then the offsets (char2) are 2-aligned, 2 * ns + 2 * nt being even,
+    // and an HBD frame stays 2-aligned, its frame_bytes and so `lead` being even.
+    const size_t lead = (4 - (p->frame_bytes + ns * 2 + nt * 2) % 4) % 4;
+    uint8_t *stage = (uint8_t *)c.take(p->frame_bytes + ns * 2 + nt * 2 + nb * 4 + 4);
+    p->d_stage = stage ? stage + lead : nullptr;
     p->d_o8_sad = p->d_stage ? (int8_t *)(p->d_stage + p->frame_bytes) : nullptr;
     p->d_o8_satd = p->d_stage ? p->d_o8_sad + ns * 2 : nullptr;
     p->d_centers = p->d_stage ? (int16_t *)(p->d_o8_satd + nt * 2) : nullptr;
@@ -214,9 +223,12 @@ extern "C" int b200_frame_pipe_create(b200_ctx *ctx, const b200_frame_pipe_cfg *
       for (int x = 0; x < nbx; x++) hb[(size_t)y * nbx + x] = b200_block{(int16_t)(x * cfg->block_w), (int16_t)(y * cfg->block_h)};
     std::vector<uint32_t> o1(nb + 1), o2(nb + 1);
     for (size_t i = 0; i <= nb; i++) o1[i] = (uint32_t)(i * cfg->sad_per_block), o2[i] = (uint32_t)(i * cfg->satd_per_block);
+    // the alignment gap between eob and tx_dist travels with the one-copy result block: zero, not stale bytes
+    const size_t gap = b200_align_up(nb * 2, 8) - nb * 2;
     if (cudaMemcpy(p->d_blocks, hb.data(), nb * sizeof(b200_block), cudaMemcpyHostToDevice) != cudaSuccess ||
         cudaMemcpy(p->d_offs_sad, o1.data(), (nb + 1) * 4, cudaMemcpyHostToDevice) != cudaSuccess ||
         cudaMemcpy(p->d_offs_satd, o2.data(), (nb + 1) * 4, cudaMemcpyHostToDevice) != cudaSuccess ||
+        (gap && cudaMemset((uint8_t *)p->d_eob + nb * 2, 0, gap) != cudaSuccess) ||
         cudaDeviceSynchronize() != cudaSuccess)
       st = b200_fail(ctx, B200_ERR_CUDA, "b200_frame_pipe_create: descriptor upload failed");
   }
@@ -420,13 +432,15 @@ extern "C" int b200_frame_pipe_push_packed(b200_frame_pipe *p, const void *frame
     pack_gather_kernel<int32_t><<<grid, 256, 0, ctx->stream>>>((const int32_t *)p->d_q, p->d_eob, p->d_pack_offs, d_scan,
                                                                coded, nb, (int32_t *)p->d_packed);
   B200_LAUNCH_CHECK(ctx);
-  // the small fixed-size results and the total
+  // the small fixed-size results and the total (the winners of a leg that is off are not written, as in a push)
   const size_t rb = nb * sizeof(b200_me_result);
-  if (best_sad && best_satd == best_sad + nb) {
+  const bool sad_leg = cfg.sad_per_block > 0, satd_leg = cfg.satd_per_block > 0;
+  if (sad_leg && satd_leg && best_sad && best_satd == best_sad + nb) {
     B200_CUDA(ctx, cudaMemcpyAsync(best_sad, p->d_best_sad, 2 * rb, cudaMemcpyDeviceToHost, ctx->stream));
   } else {
-    if (best_sad) B200_CUDA(ctx, cudaMemcpyAsync(best_sad, p->d_best_sad, rb, cudaMemcpyDeviceToHost, ctx->stream));
-    if (best_satd) B200_CUDA(ctx, cudaMemcpyAsync(best_satd, p->d_best_satd, rb, cudaMemcpyDeviceToHost, ctx->stream));
+    if (sad_leg && best_sad) B200_CUDA(ctx, cudaMemcpyAsync(best_sad, p->d_best_sad, rb, cudaMemcpyDeviceToHost, ctx->stream));
+    if (satd_leg && best_satd)
+      B200_CUDA(ctx, cudaMemcpyAsync(best_satd, p->d_best_satd, rb, cudaMemcpyDeviceToHost, ctx->stream));
   }
   if (eob) B200_CUDA(ctx, cudaMemcpyAsync(eob, p->d_eob, nb * 2, cudaMemcpyDeviceToHost, ctx->stream));
   if (tx_dist) B200_CUDA(ctx, cudaMemcpyAsync(tx_dist, p->d_dist, nb * 8, cudaMemcpyDeviceToHost, ctx->stream));

@@ -21,7 +21,8 @@ def test_example_builds_and_refuses_to_run_without_a_gpu(tmp_path):
     import torch
     exe = build(tmp_path)
     if torch.cuda.is_available():
-        pytest.skip("GPU present: covered by the gpu-marked test")
+        pytest.skip("GPU present: the run on the device is "
+                    "tests/test_frame_pipe_paths_gpu.py::test_stream_frames_example_matches_the_oracle")
     r = subprocess.run([exe, "2"], capture_output=True, text=True)
     assert r.returncode != 0 and "no CPU fallback" in r.stderr
 

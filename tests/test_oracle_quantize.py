@@ -36,7 +36,7 @@ def L():
     return l
 
 
-def chain(coeffs, tx_size, tx_type, dcq, acq, is_intra):
+def chain(coeffs, tx_size, tx_type, dcq, acq, is_intra, threads=0):
     """coeffs: (n, area) int16 or int32 -> qcoeffs, rcoeffs, eob, tx_dist"""
     l = L()
     n = len(coeffs)
@@ -48,7 +48,7 @@ def chain(coeffs, tx_size, tx_type, dcq, acq, is_intra):
     dist = np.zeros(n, np.uint64)
     l.orc_quantize_chain_batch(coeffs.ctypes.data, n, tx_size, tx_type, dcq, acq, int(is_intra),
                                int(coeffs.dtype == np.int32), q.ctypes.data, r.ctypes.data, eob.ctypes.data,
-                               dist.ctypes.data, 0)
+                               dist.ctypes.data, threads)
     return q, r, eob, dist
 
 
