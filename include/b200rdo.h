@@ -389,7 +389,7 @@ int b200_fwd_txfm_residual_multi_dev(b200_ctx *ctx, size_t npairs, const b200_pl
 /* ActivityMask::from_plane + fill_scales (activity.rs:21-100): d_variances[by * wb + bx] =
  * variance_8x8 of luma block (bx, by), wb = ceil(width / 8), hb = ceil(height / 8) (the plane's
  * padding must cover the rounding up); d_scales (may be NULL) = ssim_boost(var, var, bit_depth),
- * the Q14 DistortionScale per importance block. */
+ * the Q14 DistortionScale per importance block.  An empty plane launches nothing. */
 int b200_activity_mask_dev(b200_ctx *ctx, const b200_plane *luma, int bit_depth, uint32_t *d_variances,
                            uint32_t *d_scales);
 
@@ -460,11 +460,13 @@ int b200_frame_pipe_push_packed(b200_frame_pipe *pipe, const void *frame, ptrdif
  * dst is ((src.width + 1) / 2) x ((src.height + 1) / 2), followed by Plane::pad(frame_w, frame_h):
  * everything outside [0, pad_w) x [0, pad_h) is a replica of the nearest pixel inside, with
  * pad_w = (frame_w + xdec) >> xdec, pad_h = (frame_h + ydec) >> ydec of the NEW plane (xdec = 1 for
- * the half, 2 for the quarter resolution plane).  The whole padded area of dst is written. */
+ * the half, 2 for the quarter resolution plane).  The whole padded area of dst is written.  Both planes
+ * must share bpp 1 or 2. */
 int b200_plane_downsample_dev(b200_ctx *ctx, const b200_plane *src, const b200_plane *dst, int pad_w, int pad_h);
 /* estimate_intra_costs (lookahead.rs:30-128): for every 8x8 importance block of the source luma,
  * get_intra_edges(DC_PRED, TX_8X8) -> DC prediction -> get_satd against the source, fused;
- * d_costs[(y / 8) * (width / 8) + x / 8]. */
+ * d_costs[(y / 8) * (width / 8) + x / 8].  bit_depth must be 8 (bpp 1), 10 or 12 (bpp 2); a plane
+ * narrower or shorter than 8 pixels has no block and launches nothing. */
 int b200_estimate_intra_costs_dev(b200_ctx *ctx, const b200_plane *luma, int bit_depth, uint32_t *d_costs);
 /* The cost part of estimate_inter_costs (lookahead.rs:238-270): SATD between every importance block and
  * the reference block displaced by its motion vector (d_mvs: (row, col) int16 per importance block =
@@ -545,7 +547,8 @@ typedef struct {
 } b200_imp_step;
 /* frames: HOST array of nframes source luma planes (same size and bpp; padding covers the ceil grid
  * and wherever the vectors point, as for b200_estimate_inter_costs_dev); d_intra_costs: nframes x
- * floor(W/8)*floor(H/8); d_importances: nframes x n_imp f32, zeroed by the call, then propagated. */
+ * floor(W/8)*floor(H/8); d_importances: nframes x n_imp f32, zeroed by the call, then propagated.
+ * bit_depth must be 8 (bpp 1), 10 or 12 (bpp 2). */
 int b200_block_importances_dev(b200_ctx *ctx, size_t nframes, const b200_plane *frames, int bit_depth,
                                const uint32_t *d_intra_costs, const int16_t *d_mvs, size_t nsteps,
                                const b200_imp_step *steps, float *d_importances);
@@ -561,7 +564,7 @@ int b200_distortion_scales_dev(b200_ctx *ctx, const b200_plane *frame, const flo
  * b200_activity_mask_dev; d_spatiotemporal required).  d_scales is scaled in place;
  * *d_log_isqrt_mean_scale (may be NULL) = the returned inv_mean.blog64() >> 1; d_scale4x4 (may be NULL)
  * = sse_wxh's per-4x4-chunk luma map (rdo.rs:177-224): 2*w_imp x 2*h_imp entries, rows scale4x4_stride
- * apart, ready for b200_weighted_sse_dev. */
+ * apart, ready for b200_weighted_sse_dev.  w_imp * h_imp must be below 2^30. */
 int b200_temporal_scores_dev(b200_ctx *ctx, size_t w_imp, size_t h_imp, uint32_t *d_scales,
                              const uint32_t *d_activity, uint32_t *d_spatiotemporal,
                              int64_t *d_log_isqrt_mean_scale, uint32_t *d_scale4x4, size_t scale4x4_stride);

@@ -145,7 +145,8 @@ int check_pair(b200_ctx *ctx, const b200_plane *a, const b200_plane *b) {
 extern "C" int b200_plane_downsample_dev(b200_ctx *ctx, const b200_plane *src, const b200_plane *dst, int pad_w,
                                          int pad_h) {
   B200_REQUIRE(ctx, ctx != nullptr, "ctx is NULL");
-  B200_REQUIRE(ctx, src && dst && src->data && dst->data && src->bpp == dst->bpp, "bad planes");
+  B200_REQUIRE(ctx, src && dst && src->data && dst->data && src->bpp == dst->bpp && (src->bpp == 1 || src->bpp == 2),
+               "bad planes");
   const int w = (src->width + 1) / 2, h = (src->height + 1) / 2;
   B200_REQUIRE(ctx, dst->width == w && dst->height == h, "destination must be %d x %d (is %d x %d)", w, h, dst->width,
                dst->height);
@@ -169,8 +170,9 @@ extern "C" int b200_plane_downsample_dev(b200_ctx *ctx, const b200_plane *src, c
 extern "C" int b200_estimate_intra_costs_dev(b200_ctx *ctx, const b200_plane *luma, int bit_depth, uint32_t *d_costs) {
   B200_REQUIRE(ctx, ctx != nullptr, "ctx is NULL");
   B200_REQUIRE(ctx, luma && luma->data && d_costs, "NULL plane / output");
-  B200_REQUIRE(ctx, (luma->bpp == 1) == (bit_depth == 8) && bit_depth >= 8 && bit_depth <= 12, "bpp %d vs bit depth %d",
-               luma->bpp, bit_depth);
+  B200_REQUIRE(ctx, bit_depth == 8 || bit_depth == 10 || bit_depth == 12, "bit depth %d not in {8,10,12}", bit_depth);
+  B200_REQUIRE(ctx, (luma->bpp == 1 || luma->bpp == 2) && (luma->bpp == 1) == (bit_depth == 8),
+               "bpp %d vs bit depth %d", luma->bpp, bit_depth);
   const int wb = luma->width / 8, hb = luma->height / 8;
   if (wb == 0 || hb == 0) return B200_OK;
   B200_CUDA(ctx, cudaSetDevice(ctx->device));

@@ -271,8 +271,9 @@ extern "C" int b200_activity_mask_dev(b200_ctx *ctx, const b200_plane *luma, int
   B200_REQUIRE(ctx, luma->pad >= wb * 8 - luma->width && luma->pad >= hb * 8 - luma->height,
                "plane padding %d too small for the %dx%d region rounded up to 8", luma->pad, luma->width, luma->height);
   B200_REQUIRE(ctx, d_variances != nullptr, "NULL output");
-  B200_CUDA(ctx, cudaSetDevice(ctx->device));
   const long long n = (long long)wb * hb;
+  if (n == 0) return B200_OK;  // an empty plane: a zero-block grid is not a valid launch
+  B200_CUDA(ctx, cudaSetDevice(ctx->device));
   const int grid = (int)std::min<long long>((n + 127) / 128, (long long)ctx->num_sms * 32);
   PlaneView p{luma->data, luma->stride};
   if (luma->bpp == 1)

@@ -293,9 +293,9 @@ __global__ void scores_apply(uint32_t *scales, uint32_t *spatio, int spatio_is_p
 int check_planes(b200_ctx *ctx, size_t nframes, const b200_plane *frames, int bit_depth) {
   B200_REQUIRE(ctx, frames != nullptr && nframes > 0, "no frames");
   const b200_plane &f0 = frames[0];
-  B200_REQUIRE(ctx, (f0.bpp == 1) == (bit_depth == 8) && (f0.bpp == 1 || f0.bpp == 2) && bit_depth >= 8 &&
-                        bit_depth <= 12,
-               "bpp %d vs bit depth %d", f0.bpp, bit_depth);
+  B200_REQUIRE(ctx, bit_depth == 8 || bit_depth == 10 || bit_depth == 12, "bit depth %d not in {8,10,12}", bit_depth);
+  B200_REQUIRE(ctx, (f0.bpp == 1) == (bit_depth == 8) && (f0.bpp == 1 || f0.bpp == 2), "bpp %d vs bit depth %d",
+               f0.bpp, bit_depth);
   B200_REQUIRE(ctx, f0.width > 0 && f0.height > 0, "empty frame");
   const int w_imp = (f0.width + 7) / 8, h_imp = (f0.height + 7) / 8;
   for (size_t f = 0; f < nframes; f++) {
@@ -427,7 +427,9 @@ extern "C" int b200_temporal_scores_dev(b200_ctx *ctx, size_t w_imp, size_t h_im
                                         int64_t *d_log_isqrt_mean_scale, uint32_t *d_scale4x4,
                                         size_t scale4x4_stride) {
   B200_REQUIRE(ctx, ctx != nullptr, "ctx is NULL");
-  B200_REQUIRE(ctx, w_imp > 0 && h_imp > 0 && w_imp * h_imp < (1u << 30), "bad map size %zu x %zu", w_imp, h_imp);
+  // each side bounded first, so that the product cannot wrap
+  B200_REQUIRE(ctx, w_imp > 0 && h_imp > 0 && w_imp < (1u << 30) && h_imp < (1u << 30) && w_imp * h_imp < (1u << 30),
+               "bad map size %zu x %zu", w_imp, h_imp);
   B200_REQUIRE(ctx, d_scales != nullptr, "NULL scales");
   B200_REQUIRE(ctx, !d_activity || d_spatiotemporal, "the spatiotemporal form needs d_spatiotemporal");
   B200_REQUIRE(ctx, !d_scale4x4 || scale4x4_stride >= 2 * w_imp, "4x4 map stride %zu < %zu", scale4x4_stride,

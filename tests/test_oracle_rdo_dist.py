@@ -123,6 +123,85 @@ def test_cdef_dist_kernel_pieces():
             assert fn(s.ctypes.data, 12, s.ctypes.data, 12, w, h, bd, None) == 0
 
 
+M64 = (1 << 64) - 1
+SSIM_RATIO = (((3355 << 15) // 12338) + 1) >> 1                 # activity.rs:179
+
+
+def py_ssim_boost_rsqrt(x):
+    """activity.rs:107-143 in Python integers: ilog2, i16 k / s, the `as u16` cast, i32 arithmetic shifts
+    (Python's >> on negative ints is the arithmetic shift Rust's i32 >> is) -> (norm, shift)"""
+    k = (x.bit_length() - 1) >> 1
+    s = 2 * k - (16 - 2)
+    t = (x >> s if s > 0 else x << -s) & 0xFFFF
+    shift = (14 + ((s + 16) >> 1)) & 0xFF
+    n = t - 32768
+    rsqrt = 23557 + ((n * (-13490 + ((n * 6711) >> 15))) >> 15)
+    return rsqrt & 0xFFFF, shift
+
+
+def py_apply_ssim_boost(inp, svar, dvar, bd):
+    """activity.rs:159-186 in Python integers, wrapping u64 products and the final `as u32` like a release
+    build"""
+    cs = bd - 8
+    sv, dv = svar >> (2 * cs), dvar >> (2 * cs)
+    c1, c2, c3 = 3355, 16128, 12338
+    ratio = (((c1 << 15) // c3) + 1) >> 1
+    assert ratio == SSIM_RATIO
+    norm, shift = py_ssim_boost_rsqrt(c1 * c1 + sv * dv)
+    inner = (((ratio * (sv + dv + c2)) & M64) * norm & M64) >> 14
+    return (((inp * inner) & M64) >> shift) & 0xFFFFFFFF
+
+
+def test_apply_ssim_boost_python_restatement_equals_the_oracle():
+    """Both ends of every input: input, svar, dvar in {0, 1, ..., 2^32 - 1}, every bit depth, plus a random
+    sweep; the inputs whose u64 product wraps are among them."""
+    l = L()
+    u32_edges = [0, 1, 2, 3, 255, 256, 4095, 16128, 65535, 1 << 16, (1 << 20) - 1, 1 << 24, 268304400,
+                 (1 << 31) - 1, 1 << 31, (1 << 32) - 2, (1 << 32) - 1]
+    inputs = [0, 1, 1 << 14, (1 << 14) + 1, 268304400, (1 << 32) - 1]
+    wrapped = 0
+    for bd in (8, 10, 12):
+        for inp in inputs:
+            for sv in u32_edges:
+                for dv in u32_edges:
+                    want = l.orc_apply_ssim_boost(inp, sv, dv, bd)
+                    assert py_apply_ssim_boost(inp, sv, dv, bd) == want, (inp, sv, dv, bd)
+                    cs = bd - 8
+                    a, b = sv >> 2 * cs, dv >> 2 * cs
+                    norm, _ = py_ssim_boost_rsqrt(3355 * 3355 + a * b)
+                    wrapped += inp * (((SSIM_RATIO * (a + b + 16128)) * norm) >> 14) > M64
+    assert wrapped > 0
+    rng = np.random.default_rng(11)
+    for _ in range(20000):
+        bd = int(rng.choice([8, 10, 12]))
+        inp, sv, dv = (int(v) for v in rng.integers(0, 1 << 32, 3, dtype=np.uint64) >> rng.integers(0, 32, 3).astype(np.uint64))
+        assert py_apply_ssim_boost(inp, sv, dv, bd) == l.orc_apply_ssim_boost(inp, sv, dv, bd), (inp, sv, dv, bd)
+
+
+def parse_area_divisors(path, name):
+    """the 64 initialisers of the array `name` in a C / CUDA source"""
+    import os
+    import re
+    src = open(os.path.join(O.ROOT, path)).read()
+    body = re.search(name + r"\[64\]\s*=\s*\{(.*?)\};", re.sub(r"/\*.*?\*/", "", src, flags=re.S), re.S).group(1)
+    return [int(v) for v in re.findall(r"\d+", body)]
+
+
+def test_area_divisors_are_round_2_14_over_area_in_both_tables():
+    """kAreaDivisors (rdo_dist_dev.cuh) and the oracle's AREA_DIVISORS (rdo_dist.c) against
+    round(2^14 / (1 + x)) (dist.rs:288-297), exactly: a w x h <= 8x8 block reaches only 30 of the 64
+    entries, so this pins the rest.  No entry is a tie, so the rounding direction does not matter."""
+    from fractions import Fraction
+    want = []
+    for x in range(64):
+        q = Fraction(1 << 14, 1 + x)
+        assert q - int(q) != Fraction(1, 2)
+        want.append(int(q + Fraction(1, 2)))
+    assert parse_area_divisors("rav1e_b200/csrc/rdo_dist_dev.cuh", "kAreaDivisors") == want
+    assert parse_area_divisors("oracle/rdo_dist.c", "AREA_DIVISORS") == want
+    assert len({w * h for w in range(1, 9) for h in range(1, 9)}) == 30
+
+
 def test_distortion_scale_mul_rounds_to_nearest():
     l = L()
     assert l.orc_distortion_scale_mul(1 << 14, 12345) == 12345
