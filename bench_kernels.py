@@ -313,6 +313,118 @@ def intra_screen(ctx):
         ctx.plane_free(src)
 
 
+def cfl_alpha(ctx):
+    """b200_cfl_alpha_dev over every chroma-carrying block of each cfl_allowed size of a 1080p 4:2:0 frame (one
+    call per size, tx_size = the size's largest luma tx), and one call with all sizes mixed, 8 and 10 bit.  Next
+    to it, the same blocks through b200_pred_cfl_ac_dev + b200_get_intra_edges_dev (both planes) +
+    b200_predict_intra_dev with 33 items per (block, plane): a lower bound for the composition a caller has
+    without the fused call, since it writes every prediction to HBM and computes no SSE and no decision.  A
+    sample of every timed fused call is checked against the CPU oracle."""
+    from scipy.ndimage import uniform_filter
+    from tests.test_oracle_cfl_alpha import CFL_ITEM_DTYPE, Frame, cfl_alpha as orc_cfl_alpha, grid_items, valid
+    from tests.test_oracle_intra_edges import BSIZES
+    rng = np.random.default_rng(23)
+    W, H, PAD = 1920, 1080, 96
+    cw, ch = W // 2, H // 2
+
+    def smooth(w, h):
+        b = uniform_filter(rng.integers(0, 256, (h, w)).astype(np.float32), 5)
+        return (b - b.min()) / (b.max() - b.min())
+    luma, cb, cr = smooth(W + 32, H + 32), smooth(cw, ch), smooth(cw, ch)
+    for bd in (8, 10):
+        maxv = (1 << bd) - 1
+        dtype = np.uint8 if bd == 8 else np.uint16
+        bpp = np.dtype(dtype).itemsize
+        q = [np.rint(p * maxv).astype(dtype) for p in (luma, cb, cr)]
+        srcs = [q[0]] + [np.clip(np.rint(p * maxv + rng.normal(0, 3 * maxv / 255, p.shape)), 0, maxv).astype(dtype)
+                         for p in (cb, cr)]
+        F = Frame(q, srcs, 1, 1, W, H, bd)
+        rec = [ctx.plane_from_host(p.view(), PAD) for p in F.rec]
+        src = [ctx.plane_from_host(p.view(), PAD) for p in F.src]
+        rect = (0, 0, W, H)
+        per_size = {}
+        for bs in range(10):
+            items = grid_items(rng, rect, [bs], tx_random=False)
+            keep = np.array([valid(F, rect, int(i["x"]), int(i["y"]), bs, int(i["tx_size"])) for i in items])
+            per_size[bs] = items[keep]
+        mixed = np.concatenate([per_size[bs] for bs in range(10)])
+        mixed = mixed[rng.permutation(len(mixed))]
+        for bs in list(range(10)) + ["mixed"]:
+            items = mixed if bs == "mixed" else per_size[bs]
+            label = "mixed sizes" if bs == "mixed" else "%dx%d" % BSIZES[bs]
+            nb = len(items)
+            d_items = dev(items)
+            d_alpha = torch.empty(nb * 2, dtype=torch.uint8, device="cuda")
+            d_sse = torch.empty(nb * 66 * 8, dtype=torch.uint8, device="cuda")
+            ms = timed(lambda: ctx.cfl_alpha_dev(rec, src, 1, 1, rect, W, H, bd, d_items, nb, d_alpha, d_sse))
+            alpha = d_alpha.cpu().numpy().view(np.int8).reshape(nb, 2)
+            sse = d_sse.cpu().numpy().view(np.uint64).reshape(nb, 2, 33)
+            sample = rng.choice(nb, min(nb, 2000), replace=False)
+            want_alpha, want_sse = orc_cfl_alpha(F, rect, items[sample])
+            same = bool((alpha[sample] == want_alpha).all() and (sse[sample] == want_sse).all())
+            assert same, f"{label} {bd}-bit: b200_cfl_alpha_dev disagrees with the oracle"
+            cpu = cpu_rate(lambda: orc_cfl_alpha(F, rect, items, threads=O.host_threads()), nb)
+            bw = np.array([BSIZES[b][0] for b in items["bsize"]])
+            bh = np.array([BSIZES[b][1] for b in items["bsize"]])
+            tw, th = np.maximum(bw // 2, 4), np.maximum(bh // 2, 4)
+            # bytes per block: the luma footprint, two edge buffers, two source blocks, the 2 + 66 * 8 outputs
+            nbytes = float(np.mean((tw * th * 4 + 2 * (2 * (tw + th) + 1) + 2 * tw * th) * bpp + 2 + 66 * 8))
+            extra = {"block": label, "bit_depth": bd, "ms_per_call": ms, "oracle_sample": len(sample),
+                     "same_as_oracle": same, "alphas_evaluated_mean": float((sse != np.uint64(2**64 - 1)).sum() / nb / 2),
+                     "library": os.path.basename(B.LIB_PATH)}
+            emit(f"cfl_alpha_dev {label} {bd}-bit 4:2:0 (luma AC + 2 x (edges + 33 CfL predictions + SSE) + early "
+                 "exit, fused)", nb, "blocks", ms, nbytes, "1080p 4:2:0, every chroma-carrying block, tx = largest "
+                 "luma tx, one call; bytes: luma footprint + 2 edges + 2 source blocks + outputs", cpu=cpu, extra=extra)
+            if bs == "mixed":
+                continue
+            # the lower bound: AC, edges of both planes, 33 predictions per (block, plane) written to HBM
+            w, h = int(tw[0]), int(th[0])
+            blocks = np.zeros(nb, B.BLOCK_DTYPE)
+            blocks["x"], blocks["y"] = items["x"] - 4 * (bw == 4), items["y"] - 4 * (bh == 4)   # sub8x8_offset
+            d_blocks = dev(blocks)
+            d_ac = torch.empty(nb * w * h * 2, dtype=torch.uint8, device="cuda")
+            eit = np.zeros(nb, B.EDGE_ITEM_DTYPE)
+            eit["po_x"], eit["po_y"] = (items["x"] >> 3) << 2, (items["y"] >> 3) << 2
+            eit["part_x"], eit["part_y"] = items["x"] >> 2, items["y"] >> 2
+            eit["bsize"], eit["tx_size"], eit["mode"] = bs, TX_SIZES.index((w, h)), 13
+            d_eit = dev(eit)
+            ebytes = nb * 257 * bpp
+            d_edges = torch.empty(2 * ebytes, dtype=torch.uint8, device="cuda")
+            d_lens = torch.empty(2 * nb * 2, dtype=torch.uint8, device="cuda")
+            crect = (0, 0, cw, ch)
+            for p in (0, 1):
+                ctx.get_intra_edges_dev(rec[1 + p], crect, 1, 1, bd, d_eit, nb, d_edges[p * ebytes:],
+                                        d_lens[p * nb * 2:])
+            lens = d_lens.cpu().numpy().reshape(2, nb, 2)
+            pit = np.zeros((2, nb, 33), B.INTRA_ITEM_DTYPE)
+            al = np.arange(-16, 17)
+            px, py = eit["po_x"][None, :, None], eit["po_y"][None, :, None]
+            pit["edge"] = np.arange(2)[:, None, None] * nb + np.arange(nb)[None, :, None]
+            pit["ac"] = np.arange(nb)[None, :, None]
+            pit["x"], pit["y"] = px, py
+            pit["angle"], pit["mode"] = al[None, None, :], np.where(al == 0, 0, 13)[None, None, :]
+            pit["variant"] = np.where((px == 0) & (py == 0), 0, np.where(py == 0, 1, np.where(px == 0, 2, 3)))
+            pit["ief"] = -1
+            pit["left_len"], pit["above_len"] = lens[:, :, 0][:, :, None], lens[:, :, 1][:, :, None]
+            d_pit = dev(pit.reshape(-1))
+            d_pred = torch.empty(2 * nb * 33 * w * h * bpp, dtype=torch.uint8, device="cuda")
+
+            def composed():
+                ctx.pred_cfl_ac_dev(rec[0], d_blocks, nb, w, h, 0, 0, 1, 1, d_ac)
+                for p in (0, 1):
+                    ctx.get_intra_edges_dev(rec[1 + p], crect, 1, 1, bd, d_eit, nb, d_edges[p * ebytes:],
+                                            d_lens[p * nb * 2:])
+                ctx.predict_intra_dev(d_edges, d_pit, 2 * nb * 33, d_ac, w, h, bd, cw, ch, d_pred)
+            ms2 = timed(composed)
+            emit(f"pred_cfl_ac_dev + get_intra_edges_dev x2 + predict_intra_dev x66 {label} {bd}-bit 4:2:0 (lower "
+                 "bound of the unfused composition)", nb, "blocks", ms2, nbytes + 66 * w * h * bpp,
+                 "same blocks; the 66 predictions per block written to HBM, no SSE and no decision (the library has "
+                 "no SSE over packed predictions), so a lower bound for today's composition",
+                 extra={"block": label, "bit_depth": bd, "ms_per_call": ms2, "fused_speedup": ms2 / ms})
+        for p in rec + src:
+            ctx.plane_free(p)
+
+
 def inter_screen(ctx):
     """b200_inter_mode_screen_dev over every block of a 1080p frame (one call per size), 8 and 10 bit, on
     lists from the mode-list model (rdo.rs:1158-1318) for two references, one forward and one backward, with
@@ -542,6 +654,9 @@ def main():
         return
     if "--cdef-rdo" in sys.argv[1:]:
         cdef_rdo(ctx)
+        return
+    if "--cfl-alpha" in sys.argv[1:]:
+        cfl_alpha(ctx)
         return
     rng = np.random.default_rng(0)
     W, H, PAD = 1920, 1080, 96

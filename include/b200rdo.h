@@ -891,6 +891,51 @@ int b200_pred_cfl_ac_dev(b200_ctx *ctx, const b200_plane *luma, const b200_block
                          size_t nblocks, int bw, int bh, int w_pad, int h_pad, int xdec, int ydec,
                          int16_t *d_ac);
 
+/* The CfL alpha search of rdo_mode_decision (rdo.rs:1013-1041): rdo_cfl_alpha (rdo.rs:1593-1689) for a batch
+ * of blocks of one tile in one asynchronous call on the context's stream, without host synchronisation.  Per
+ * item: uv_tx_size = bsize.largest_chroma_tx_size; the visible chroma area from clip_visible_bsize
+ * (rdo.rs:228-253) at the frame block offset, i.e. ((x + rect_x) >> xdec, (y + rect_y) >> ydec), which for a
+ * sub-8x8 block at an odd 4x4 position is 2 (mod 4), not the 4-aligned chroma origin; luma_ac
+ * (predict.rs:644-698: the luma of tile_bo + sub8x8_offset, frame_clipped_bw / bh against fi.w_in_b /
+ * fi.h_in_b, the frame rounded up to 8, max_luma_w / h rounded up to the luma tx size for sides above 8,
+ * per-block w_pad / h_pad); per chroma plane get_intra_edges (UV_CFL_PRED, po = tile_bo.plane_offset),
+ * predict_intra at each alpha -16 ..= 16 (alpha 0 = DC_PRED, else DC + get_scaled_luma_q0) and sse_wxh over
+ * the visible area at the default DistortionScale (whole 4x4 chunks only); then the reference's early exit:
+ * best = (cost(0), 0), count = 2, for alpha 1..=16 +alpha then -alpha against the updated best, each strict
+ * improvement adds 2 to count, break when count < alpha.  Predictions exist only in registers; `rec` is not
+ * written (the reference's last write there is dead: its caller re-predicts chroma, rdo.rs:1054-1075).
+ *
+ * rec / src: HOST arrays of the three frame planes (src[0] is not read).  (rect_x, rect_y, rect_w, rect_h) is
+ * the tile in luma pixels, origin a multiple of 8, inside the frame's 8x8 blocks; the chroma region is that
+ * rect decimated (TileRect::decimated).  frame_width / frame_height = fi.width / fi.height.  What may share a
+ * call is the caller's business: each block's luma reconstruction and its chroma neighbours must be final in
+ * rec (one wavefront of the encode loop); tiles run on their own threads and contexts (encoder.rs:3253).
+ *
+ * d_alpha (nitems x 2: best_alpha of planes 1 and 2; the caller forms None when both are 0, else
+ * CFLParams::from_alpha) and d_sse (nitems x 2 x 33, [item][plane - 1][alpha + 16]: the sse_wxh of every alpha
+ * the reference evaluates, UINT64_MAX for the alphas its loop never reaches) may each be NULL, not both.
+ * Rejected with B200_ERR_ARG before any launch: NULL pointers, a bit depth other than 8 / 10 / 12 or a bpp
+ * that does not match it, a layout other than 4:2:0 / 4:2:2 / 4:4:4, planes smaller than the frame (chroma:
+ * (fi.width + xdec) >> xdec by (fi.height + ydec) >> ydec), src and rec chroma of different sizes, a region
+ * outside the frame's 8x8 blocks or not 8-aligned, and a luma rec that does not reach 31 pixels past the
+ * frame in each direction (rec[0].width + rec[0].pad >= frame_width + 31, likewise the height: luma_ac reads
+ * up to that far past the visible frame, as the reference does).  nitems == 0 launches nothing.
+ * An invalid item gets {0, 0} in d_alpha and UINT64_MAX in its 66 d_sse entries, and nothing is read for it:
+ * bsize > BLOCK_32X32 (cfl_allowed; 4x16 / 16x4 / 8x32 / 32x8 included), a size with no subsampled_size for
+ * the layout (4:2:2: 4x8, 8x16, 16x32), a block without chroma (has_chroma), tx_size >= 19 or larger than
+ * the block, (x, y) outside the region or not a multiple of 4.  A valid item whose visible area is 0 gets the
+ * same outputs (the reference returns None without evaluating anything). */
+typedef struct {
+  int16_t x, y;    /* block's top-left inside the region, luma px, multiples of 4 (tile_bo.to_luma_plane_offset) */
+  uint8_t bsize;   /* BlockSize 0..21; only cfl_allowed() sizes (discriminant <= BLOCK_32X32) are valid */
+  uint8_t tx_size; /* the block's luma TxSize (rdo_mode_decision's best.tx_size) */
+  uint8_t pad_[2];
+} b200_cfl_item; /* 8 B */
+int b200_cfl_alpha_dev(b200_ctx *ctx, const b200_plane rec[3], const b200_plane src[3], int xdec, int ydec,
+                       int rect_x, int rect_y, int rect_w, int rect_h, int frame_width, int frame_height,
+                       int bit_depth, const b200_cfl_item *d_items, size_t nitems, int8_t *d_alpha,
+                       uint64_t *d_sse);
+
 /* ------------------------------------------------ reference-signature symbols (MC / intra / CDEF)
  * The reference's own extern "C" prototypes, symbol for symbol, with the ISA suffix replaced by
  * `_cuda`: they slot into PUT_FNS / PUT_HBD_FNS / PREP_FNS / PREP_HBD_FNS / AVG_FNS / AVG_HBD_FNS

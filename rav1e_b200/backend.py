@@ -95,6 +95,9 @@ INTER_SCREEN_CAND_DTYPE = np.dtype([("mv", "<i2", (2, 2)), ("ref", "u1", (2,)), 
 INTER_SCREEN_ITEM_DTYPE = np.dtype([("x", "<i2"), ("y", "<i2"), ("bsize", "u1"), ("n", "u1"), ("pad_", "u1", (2,)),
                                     ("cands", INTER_SCREEN_CAND_DTYPE, (20,))])
 assert INTER_SCREEN_CAND_DTYPE.itemsize == 12 and INTER_SCREEN_ITEM_DTYPE.itemsize == 248
+CFL_ITEM_DTYPE = np.dtype([("x", "<i2"), ("y", "<i2"), ("bsize", "u1"), ("tx_size", "u1"), ("pad_", "u1", (2,))])
+assert CFL_ITEM_DTYPE.itemsize == 8
+CFL_ALPHAS = 33              # b200_cfl_alpha_dev's d_sse entries per (item, chroma plane): alpha -16 ..= 16
 INTER_SCREEN_SINGLE = 0xFF   # b200_inter_screen_cand.ref[1] of a single-reference entry (NONE_FRAME)
 ME_RESULT_DTYPE = np.dtype(
     {"names": ["cost", "sad", "mv_row", "mv_col"],
@@ -247,6 +250,7 @@ def lib():
     L.b200_intra_mode_screen_dev.argtypes = [vp, pp, pp] + [i32] * 6 + [vp, sz, vp, vp]
     L.b200_inter_mode_screen_dev.argtypes = [vp, pp] + [i32] * 4 + [vp] + [i32] * 5 + [vp, sz, vp, vp]
     L.b200_cdef_rdo_dev.argtypes = [vp, vp, vp, vp] + [i32] * 8 + [vp] * 5 + [C.c_double, vp, sz, vp, vp, vp, vp]
+    L.b200_cfl_alpha_dev.argtypes = [vp, vp, vp] + [i32] * 9 + [vp, sz, vp, vp]
     _LIB = L
     return L
 
@@ -558,6 +562,20 @@ class Context:
                                                      C.addressof(arr), len(refs), xorigin, yorigin, filter_mode,
                                                      bit_depth, _dev_ptr(d_items), n, _dev_ptr(d_satd),
                                                      _dev_ptr(d_order)))
+
+    def cfl_alpha_dev(self, rec, src, xdec, ydec, rect, width, height, bit_depth, d_items, n, d_alpha, d_sse):
+        """rec / src: lists of the 3 frame Planes (src[0] is not read); rect = (x, y, w, h) of the tile in luma
+        pixels; width / height = fi.width / fi.height; d_items: CFL_ITEM_DTYPE on the device; d_alpha (n x 2 i8)
+        and d_sse (n x 2 x 33 u64) may each be None (include/b200rdo.h)."""
+        def arr(planes):
+            a = (Plane * 3)()
+            for k, p in enumerate(planes):
+                C.memmove(C.byref(a[k]), C.byref(p), C.sizeof(Plane))
+            return a
+        r, s_ = arr(rec), arr(src)
+        self.check(self.L.b200_cfl_alpha_dev(self.h, C.addressof(r), C.addressof(s_), xdec, ydec, rect[0], rect[1],
+                                             rect[2], rect[3], width, height, bit_depth, _dev_ptr(d_items), n,
+                                             _dev_ptr(d_alpha), _dev_ptr(d_sse)))
 
     def pred_cfl_ac_dev(self, luma, d_blocks, n, bw, bh, w_pad, h_pad, xdec, ydec, d_ac):
         self.check(self.L.b200_pred_cfl_ac_dev(self.h, C.byref(luma), _dev_ptr(d_blocks), n, bw, bh,

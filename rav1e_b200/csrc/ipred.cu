@@ -54,11 +54,7 @@ __global__ void __launch_bounds__(128) ipred_kernel(IpredArgs a) {
     for (int i = threadIdx.x; i < w * h; i += blockDim.x) {
       const int r = i / w, c = i - r * w;
       int v = ipred_pixel(p, r, c);
-      if (ac) {  // pred_cfl_inner, predict.rs:1065-1088 + get_scaled_luma_q0 :626-635
-        const int q6 = (int)alpha * (int)ac[i];
-        const int q0 = (abs(q6) + 32) >> 6;
-        v = min(max(v + (q6 < 0 ? -q0 : q0), 0), maxv);
-      }
+      if (ac) v = cfl_pixel(v, alpha, ac[i], maxv);  // pred_cfl_inner, predict.rs:1065-1088
       out[i] = (T)v;
     }
   }
@@ -78,24 +74,15 @@ template <typename T>
 __global__ void __launch_bounds__(128) cfl_ac_kernel(CflAcArgs a) {
   __shared__ int s_sum[4];
   __shared__ int s_avg;
-  const int bw = a.bw, bh = a.bh, xdec = a.xdec, ydec = a.ydec;
-  const int max_luma_x = max((bw - a.w_pad * 4) << xdec, 8) - (1 << xdec);
-  const int max_luma_y = max((bh - a.h_pad * 4) << ydec, 8) - (1 << ydec);
-  int shift = 0;
-  for (int v = bw; v > 1; v >>= 1) shift++;
-  for (int v = bh; v > 1; v >>= 1) shift++;
+  const int bw = a.bw, bh = a.bh;
+  const CflAcShape shape = cfl_ac_shape(bw, bh, a.w_pad, a.h_pad, a.xdec, a.ydec);
   for (size_t blk = blockIdx.x; blk < a.n; blk += gridDim.x) {
     const b200_block b = a.blocks[blk];
     const T *luma = (const T *)a.luma + (long long)b.y * a.stride + b.x;
     short *ac = a.ac + blk * (size_t)bw * bh;
     int local = 0;
     for (int i = threadIdx.x; i < bw * bh; i += blockDim.x) {
-      const int sy = i / bw, sx = i - sy * bw;
-      const int y = min(sy << ydec, max_luma_y), x = min(sx << xdec, max_luma_x);
-      short s = (short)luma[(long long)y * a.stride + x];
-      if (xdec) s = (short)(s + (short)luma[(long long)y * a.stride + x + 1]);
-      if (ydec) s = (short)(s + (short)luma[(long long)(y + 1) * a.stride + x] + (short)luma[(long long)(y + 1) * a.stride + x + 1]);
-      s = (short)(s << (3 - xdec - ydec));
+      const short s = cfl_ac_sample(shape, luma, a.stride, i);
       ac[i] = s;
       local += s;
     }
@@ -106,7 +93,7 @@ __global__ void __launch_bounds__(128) cfl_ac_kernel(CflAcArgs a) {
     if (threadIdx.x == 0) {
       int sum = 0;
       for (int k = 0; k < (int)(blockDim.x >> 5); k++) sum += s_sum[k];
-      s_avg = (short)((sum + (1 << (shift - 1))) >> shift);
+      s_avg = cfl_ac_average(shape, sum);
     }
     __syncthreads();
     const short avg = (short)s_avg;

@@ -1,5 +1,6 @@
 // ipred_dev.cuh — the device form of dispatch_predict_intra (rav1e src/predict.rs:705-1505), shared by
-// the batched predictor (ipred.cu) and the intra mode screening (intra_screen.cu).
+// the batched predictor (ipred.cu), the intra mode screening (intra_screen.cu) and the CfL alpha search
+// (cfl_alpha.cu, which also shares pred_cfl_ac with ipred.cu's cfl_ac_kernel).
 //
 // A prediction is split in two so that a kernel can evaluate any pixel of it anywhere:
 //   - preparation, once per (block, mode) by a group of threads: the DC value (ipred_dc, one thread)
@@ -348,6 +349,49 @@ __device__ __forceinline__ auto ipred_dispatch(const IpredPix &p, F &&f) {
 // The predicted pixel at row r, column c of any prediction.
 __device__ __forceinline__ int ipred_pixel(const IpredPix &p, int r, int c) {
   return ipred_dispatch(p, [&](auto k) { return ipred_pixel_k<decltype(k)::value>(p, r, c); });
+}
+
+// ---- chroma from luma (shared by ipred.cu's CfL kernels and the CfL alpha search, cfl_alpha.cu)
+
+// pred_cfl_inner (predict.rs:1065-1088) for one pixel of a non-zero alpha, with get_scaled_luma_q0
+// (:626-635): the DC value plus the scaled luma AC, clamped to the bit depth.
+__device__ __forceinline__ int cfl_pixel(int dc, int alpha, int ac, int maxv) {
+  const int q6 = alpha * ac;
+  const int q0 = (abs(q6) + 32) >> 6;
+  return min(max(dc + (q6 < 0 ? -q0 : q0), 0), maxv);
+}
+
+// pred_cfl_ac (predict.rs:1020-1063) for a bw x bh chroma block with its padding: the clamp limits
+// of the luma reads and the log2 area the average divides by.
+struct CflAcShape {
+  int bw, xdec, ydec, max_luma_x, max_luma_y, shift;
+};
+__device__ __forceinline__ CflAcShape cfl_ac_shape(int bw, int bh, int w_pad, int h_pad, int xdec, int ydec) {
+  CflAcShape s;
+  s.bw = bw;
+  s.xdec = xdec;
+  s.ydec = ydec;
+  s.max_luma_x = max((bw - w_pad * 4) << xdec, 8) - (1 << xdec);
+  s.max_luma_y = max((bh - h_pad * 4) << ydec, 8) - (1 << ydec);
+  s.shift = 0;
+  for (int v = bw; v > 1; v >>= 1) s.shift++;
+  for (int v = bh; v > 1; v >>= 1) s.shift++;
+  return s;
+}
+// Element i (raster order) of the block before the average is removed: the subsampled luma sum << 3 - xdec - ydec,
+// in the reference's i16 arithmetic.  `luma` addresses the block's luma pixel (0, 0).
+template <typename T>
+__device__ __forceinline__ short cfl_ac_sample(const CflAcShape &s, const T *luma, int stride, int i) {
+  const int sy = i / s.bw, sx = i - sy * s.bw;
+  const int y = min(sy << s.ydec, s.max_luma_y), x = min(sx << s.xdec, s.max_luma_x);
+  short v = (short)luma[(long long)y * stride + x];
+  if (s.xdec) v = (short)(v + (short)luma[(long long)y * stride + x + 1]);
+  if (s.ydec) v = (short)(v + (short)luma[(long long)(y + 1) * stride + x] + (short)luma[(long long)(y + 1) * stride + x + 1]);
+  return (short)(v << (3 - s.xdec - s.ydec));
+}
+// The average the reference subtracts, from the i32 sum of the samples.
+__device__ __forceinline__ short cfl_ac_average(const CflAcShape &s, int sum) {
+  return (short)((sum + (1 << (s.shift - 1))) >> s.shift);
 }
 
 }  // namespace ipred
