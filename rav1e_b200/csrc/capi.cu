@@ -1,7 +1,7 @@
 // capi.cu — context, memory and plane management of the C ABI (include/b200rdo.h).
 #include <mutex>
 
-#include "common.cuh"
+#include "host_stage.cuh"
 
 char g_b200_last_error[512] = {0};
 
@@ -151,10 +151,8 @@ b200_ctx *b200_default_ctx() {
   if (!t.ctx) {
     int dev = 0;
     if (const char *e = getenv("B200RDO_DEVICE")) dev = atoi(e);
-    if (b200_ctx_create(dev, &t.ctx) != B200_OK) {
-      fprintf(stderr, "b200rdo: FATAL: %s\n", g_b200_last_error);
-      abort();  // no CPU fallback, by design
-    }
+    // no CPU fallback, by design; the failure is recorded in the global last error
+    b200_percall_check(nullptr, b200_ctx_create(dev, &t.ctx), "context creation");
   }
   return t.ctx;
 }
@@ -245,22 +243,12 @@ extern "C" int b200_plane_upload(b200_ctx *ctx, const b200_plane *p, const void 
   if ((size_t)host_stride_bytes == row_bytes) {
     // contiguous source: ONE linear copy (a pitched copy is a DMA descriptor per row and reaches a
     // fraction of the link rate), then unpack + replicate the border on the device
-    void *packed = nullptr;
     const size_t bytes = row_bytes * p->height;
-    B200_CUDA(ctx, cudaMallocAsync(&packed, bytes, ctx->stream));
-    cudaError_t e = cudaMemcpyAsync(packed, host, bytes, cudaMemcpyHostToDevice, ctx->stream);
-    if (e == cudaSuccess) {
-      if (p->bpp == 1)
-        unpack_pad_plane_kernel<uint8_t><<<ctx->num_sms * 4, 256, 0, ctx->stream>>>(
-            (uint8_t *)p->data, p->stride, p->width, p->height, p->pad, (const uint8_t *)packed);
-      else
-        unpack_pad_plane_kernel<uint16_t><<<ctx->num_sms * 4, 256, 0, ctx->stream>>>(
-            (uint16_t *)p->data, p->stride, p->width, p->height, p->pad, (const uint16_t *)packed);
-      ctx->launches++;
-      e = cudaGetLastError();
-    }
-    cudaFreeAsync(packed, ctx->stream);
-    B200_CUDA(ctx, e);
+    HostStage s(ctx, bytes);
+    uint8_t *packed = s.take(bytes);
+    s.up(packed, host, bytes);
+    if (s.ok()) s.run(b200_plane_unpack_internal(ctx, p, packed));
+    if (int st = s.finish(false)) return st;
   } else {
     B200_CUDA(ctx, cudaMemcpy2DAsync(p->data, (size_t)p->stride * p->bpp, host,
                                      (size_t)host_stride_bytes, row_bytes, p->height,

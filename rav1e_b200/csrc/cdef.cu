@@ -12,6 +12,7 @@
 #include <algorithm>
 
 #include "cdef_dev.cuh"
+#include "host_stage.cuh"
 
 namespace {
 
@@ -297,34 +298,36 @@ extern "C" int b200_cdef_tiles_dev(b200_ctx *ctx, const b200_cdef_item *items, s
 extern "C" int32_t b200_cdef_dir(const void *img, ptrdiff_t stride, uint32_t *var, int bit_depth) {
   b200_ctx *ctx = b200_default_ctx();
   const int bpp = bit_depth == 8 ? 1 : 2;
-  void *dbase = nullptr;
-  int st = B200_OK;
-  if (cudaSetDevice(ctx->device) != cudaSuccess ||
-      cudaMallocAsync(&dbase, 64 * bpp + 256 + 64, ctx->stream) != cudaSuccess)
-    st = b200_fail(ctx, B200_ERR_CUDA, "alloc failed");
-  uint8_t *d_dir = (uint8_t *)dbase + 256;
-  int32_t *d_var = (int32_t *)((uint8_t *)dbase + 256 + 16);
-  if (!st && cudaMemcpy2DAsync(dbase, 8 * bpp, img, (size_t)stride, 8 * bpp, 8, cudaMemcpyHostToDevice,
-                               ctx->stream) != cudaSuccess)
-    st = b200_fail(ctx, B200_ERR_CUDA, "H2D copy failed");
-  if (!st) {
-    b200_plane p{dbase, 8, 8, 8, 0, bpp, nullptr};
-    st = b200_cdef_find_dir_dev(ctx, &p, bit_depth, nullptr, d_dir, d_var);
+  HostStage s(ctx, 3 * 256);
+  uint8_t *d_img = s.take(64 * bpp), *d_dir = s.take(1);
+  int32_t *d_var = (int32_t *)s.take(4);
+  s.up2d(d_img, 8 * bpp, img, (size_t)stride, 8 * bpp, 8);
+  if (s.ok()) {
+    b200_plane p{d_img, 8, 8, 8, 0, bpp, nullptr};
+    s.run(b200_cdef_find_dir_dev(ctx, &p, bit_depth, nullptr, d_dir, d_var));
   }
   uint8_t dir = 0;
   int32_t v = 0;
-  if (!st && (cudaMemcpyAsync(&dir, d_dir, 1, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-              cudaMemcpyAsync(&v, d_var, 4, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess))
-    st = b200_fail(ctx, B200_ERR_CUDA, "D2H copy failed");
-  if (dbase) cudaFreeAsync(dbase, ctx->stream);
-  if (!st && cudaStreamSynchronize(ctx->stream) != cudaSuccess) st = b200_fail(ctx, B200_ERR_CUDA, "sync failed");
-  if (st) {
-    fprintf(stderr, "b200rdo: FATAL: cdef_dir failed: %s\n", b200_last_error(ctx));
-    abort();
-  }
+  s.down(&dir, d_dir, 1);
+  s.down(&v, d_var, 4);
+  b200_percall_check(ctx, s.finish(true), "cdef_dir");
   *var = (uint32_t)v;
   return dir;
 }
+
+namespace {
+int cdef_filter_tmp16(b200_ctx *ctx, void *d_dst, const uint16_t *d_tmp, int tw, int pri_strength, int sec_strength,
+                      int dir, int damping, int bit_depth, int xsize, int ysize) {
+  if (bit_depth == 8)
+    cdef_filter_tmp16_kernel<uint8_t><<<1, 64, 0, ctx->stream>>>((uint8_t *)d_dst, xsize, d_tmp, tw, pri_strength,
+                                                                 sec_strength, dir, damping, bit_depth, xsize, ysize);
+  else
+    cdef_filter_tmp16_kernel<uint16_t><<<1, 64, 0, ctx->stream>>>((uint16_t *)d_dst, xsize, d_tmp, tw, pri_strength,
+                                                                  sec_strength, dir, damping, bit_depth, xsize, ysize);
+  B200_LAUNCH_CHECK(ctx);
+  return B200_OK;
+}
+}  // namespace
 
 extern "C" void b200_cdef_filter_block(void *dst, ptrdiff_t dst_stride, const uint16_t *tmp,
                                        ptrdiff_t tmp_stride, int pri_strength, int sec_strength,
@@ -333,36 +336,16 @@ extern "C" void b200_cdef_filter_block(void *dst, ptrdiff_t dst_stride, const ui
   const int bpp = bit_depth == 8 ? 1 : 2;
   const int xsize = 8 >> xdec, ysize = 8 >> ydec;
   const int tw = xsize + 4, th = ysize + 4;
-  void *dbase = nullptr;
-  int st = B200_OK;
-  if (cudaSetDevice(ctx->device) != cudaSuccess ||
-      cudaMallocAsync(&dbase, 512 + 64 * bpp, ctx->stream) != cudaSuccess)
-    st = b200_fail(ctx, B200_ERR_CUDA, "alloc failed");
+  HostStage s(ctx, 512 + 64 * bpp);
+  uint16_t *d_tile = (uint16_t *)s.take((size_t)tw * th * 2);
+  uint8_t *d_dst = s.take(64 * bpp);
   // the caller's pointer addresses the block's top-left inside the padded tile (2 px border);
   // tmp_stride is in BYTES like every asm-ABI stride
   const uint8_t *h0 = (const uint8_t *)tmp - 2 * tmp_stride - 2 * 2;
-  if (!st && cudaMemcpy2DAsync(dbase, tw * 2, h0, (size_t)tmp_stride, tw * 2, th, cudaMemcpyHostToDevice,
-                               ctx->stream) != cudaSuccess)
-    st = b200_fail(ctx, B200_ERR_CUDA, "H2D copy failed");
-  void *d_dst = (uint8_t *)dbase + 512;
-  if (!st) {
-    const uint16_t *d_tmp = (const uint16_t *)dbase + 2 * tw + 2;
-    if (bpp == 1)
-      cdef_filter_tmp16_kernel<uint8_t><<<1, 64, 0, ctx->stream>>>((uint8_t *)d_dst, xsize, d_tmp, tw, pri_strength,
-                                                                   sec_strength, dir, damping, bit_depth, xsize, ysize);
-    else
-      cdef_filter_tmp16_kernel<uint16_t><<<1, 64, 0, ctx->stream>>>((uint16_t *)d_dst, xsize, d_tmp, tw, pri_strength,
-                                                                    sec_strength, dir, damping, bit_depth, xsize, ysize);
-    ctx->launches++;
-    if (cudaGetLastError() != cudaSuccess) st = b200_fail(ctx, B200_ERR_CUDA, "launch failed");
-  }
-  if (!st && cudaMemcpy2DAsync(dst, (size_t)dst_stride, d_dst, xsize * bpp, xsize * bpp, ysize,
-                               cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess)
-    st = b200_fail(ctx, B200_ERR_CUDA, "D2H copy failed");
-  if (dbase) cudaFreeAsync(dbase, ctx->stream);
-  if (!st && cudaStreamSynchronize(ctx->stream) != cudaSuccess) st = b200_fail(ctx, B200_ERR_CUDA, "sync failed");
-  if (st) {
-    fprintf(stderr, "b200rdo: FATAL: cdef_filter_block failed: %s\n", b200_last_error(ctx));
-    abort();
-  }
+  s.up2d(d_tile, tw * 2, h0, (size_t)tmp_stride, tw * 2, th);
+  if (s.ok())
+    s.run(cdef_filter_tmp16(ctx, d_dst, d_tile + 2 * tw + 2, tw, pri_strength, sec_strength, dir, damping, bit_depth,
+                            xsize, ysize));
+  s.down2d(dst, (size_t)dst_stride, d_dst, xsize * bpp, xsize * bpp, ysize);
+  b200_percall_check(ctx, s.finish(true), "cdef_filter_block");
 }

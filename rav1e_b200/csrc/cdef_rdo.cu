@@ -269,8 +269,7 @@ __global__ void __launch_bounds__(kRdoThreads, 2)
 template <typename T, int XDEC, int YDEC>
 int cdef_rdo_launch(b200_ctx *ctx, const CdefRdoArgs &a, const CdefRdoSlots &s, int nslots) {
   constexpr size_t bytes = RdoLayout<XDEC, YDEC>::BYTES;
-  B200_CUDA(ctx, cudaFuncSetAttribute(cdef_rdo_kernel<T, XDEC, YDEC>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)bytes));
+  if (int st = b200_smem_opt_in(ctx, (const void *)cdef_rdo_kernel<T, XDEC, YDEC>, (int)bytes)) return st;
   cdef_rdo_kernel<T, XDEC, YDEC><<<nslots, kRdoThreads, bytes, ctx->stream>>>(a, s);
   B200_LAUNCH_CHECK(ctx);
   return B200_OK;

@@ -10,6 +10,7 @@
 #include <cstring>
 #include <map>
 #include <string>
+#include <unordered_map>
 #include <vector>
 
 #include "../../include/b200rdo.h"
@@ -31,6 +32,8 @@ struct b200_ctx {
   // stream-ordered on `stream`).
   std::map<int, uint16_t *> scan_dev;
   std::map<int, std::vector<uint16_t>> scan_host;
+  // dynamic shared memory each kernel has been opted in to on this context's device (b200_smem_opt_in)
+  std::unordered_map<const void *, int> smem_opt_in;
   char err[512] = {0};
 };
 
@@ -67,6 +70,25 @@ inline int b200_fail(b200_ctx *ctx, int status, const char *fmt, ...) {
     (ctx)->launches++;                  \
     B200_CUDA((ctx), cudaGetLastError()); \
   } while (0)
+
+// Opt `kernel` in to `bytes` of dynamic shared memory on the context's device (the current device
+// of every `_dev` call).  The attribute belongs to the device, so it is remembered per context,
+// which serves one device and one host thread.
+inline int b200_smem_opt_in(b200_ctx *ctx, const void *kernel, int bytes) {
+  int &set = ctx->smem_opt_in[kernel];
+  if (set >= bytes) return B200_OK;
+  B200_CUDA(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+  set = bytes;
+  return B200_OK;
+}
+
+// Per-call (reference-signature) forms have no error return (the reference asserts or panics; never
+// silently wrong): a failed status prints the failing step and the context's last error, then aborts.
+inline void b200_percall_check(const b200_ctx *ctx, int st, const char *what) {
+  if (st == B200_OK) return;
+  fprintf(stderr, "b200rdo: FATAL: %s failed: %s\n", what, b200_last_error(ctx));
+  abort();
+}
 
 // Grow-only device scratch.
 int b200_reserve_dwork(b200_ctx *ctx, size_t bytes);

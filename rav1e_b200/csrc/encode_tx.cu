@@ -18,8 +18,6 @@
 // `rec` must already hold that prediction in the blocks' areas (predict-then-add, like the reference
 // writes the prediction into `rec` before reconstructing).  Entropy coding of the quantized
 // coefficients (write_coeffs_lv_map) and the rate / bias terms stay with the caller.
-#include <mutex>
-
 #include "fwd_txfm_dev.cuh"
 #include "inv_txfm_dev.cuh"
 #include "quantize_dev.cuh"
@@ -144,12 +142,7 @@ int launch_enc(b200_ctx *ctx, const EncArgs &a, int hbd) {
   const auto go = [&](auto tag) -> int {
     using CoefT = decltype(tag);
     using L = EncLayout<W, H, CoefT>;
-    static std::once_flag once;
-    static cudaError_t err = cudaSuccess;
-    std::call_once(once, [] {
-      err = cudaFuncSetAttribute(encode_tx_kernel<W, H, CoefT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L::SMEM);
-    });
-    B200_CUDA(ctx, err);
+    if (int st = b200_smem_opt_in(ctx, (const void *)encode_tx_kernel<W, H, CoefT>, (int)L::SMEM)) return st;
     const size_t ctas = (a.n + L::PER - 1) / L::PER;
     const int grid = (int)std::min<size_t>(ctas, (size_t)ctx->num_sms * 16);
     encode_tx_kernel<W, H, CoefT><<<grid, kEncThreads, L::SMEM, ctx->stream>>>(a);

@@ -10,6 +10,7 @@
 // would diverge on every step, while a thread-per-vector layout needs no communication at all
 // inside a 1-D pass.
 #include "fwd_txfm_dev.cuh"
+#include "host_stage.cuh"
 
 namespace {
 
@@ -322,23 +323,15 @@ extern "C" int b200_fwd_txfm_batch(b200_ctx *ctx, const int16_t *input, size_t i
   const int w = kTxW[tx_size], h = kTxH[tx_size];
   const size_t in_elems = (nblocks - 1) * in_block_stride + (size_t)(h - 1) * in_row_stride + w;
   const size_t out_bytes = nblocks * (size_t)w * h * (coeff_is_i32 ? 4 : 2);
-  B200_CUDA(ctx, cudaSetDevice(ctx->device));
-  void *dbase = nullptr;
-  const size_t in_bytes = b200_align_up(in_elems * 2, 256);
-  B200_CUDA(ctx, cudaMallocAsync(&dbase, in_bytes + out_bytes, ctx->stream));
-  int st = B200_OK;
-  if (cudaMemcpyAsync(dbase, input, in_elems * 2, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess)
-    st = b200_fail(ctx, B200_ERR_CUDA, "H2D copy failed");
-  uint8_t *d_out = (uint8_t *)dbase + in_bytes;
-  if (!st)
-    st = b200_fwd_txfm_dev(ctx, (const int16_t *)dbase, in_block_stride, in_row_stride, d_out,
-                           nblocks, tx_size, tx_type, bd, coeff_is_i32);
-  if (!st && cudaMemcpyAsync(output, d_out, out_bytes, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess)
-    st = b200_fail(ctx, B200_ERR_CUDA, "D2H copy failed");
-  cudaFreeAsync(dbase, ctx->stream);
-  if (st) return st;
-  if (!ctx->async_batch) B200_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  return B200_OK;
+  HostStage s(ctx, b200_align_up(in_elems * 2, 256) + out_bytes);
+  int16_t *d_in = (int16_t *)s.take(in_elems * 2);
+  uint8_t *d_out = s.take(out_bytes);
+  s.up(d_in, input, in_elems * 2);
+  if (s.ok())
+    s.run(b200_fwd_txfm_dev(ctx, d_in, in_block_stride, in_row_stride, d_out, nblocks, tx_size, tx_type, bd,
+                            coeff_is_i32));
+  s.down(output, d_out, out_bytes);
+  return s.finish(!ctx->async_batch);
 }
 
 extern "C" int b200_fwd_txfm_residual_resident(b200_ctx *ctx, const b200_plane *cur,
@@ -354,25 +347,15 @@ extern "C" int b200_fwd_txfm_residual_resident(b200_ctx *ctx, const b200_plane *
   const size_t out_bytes = nblocks * area * (cur->bpp == 2 ? 4 : 2);
   const size_t blk_bytes = b200_align_up(nblocks * sizeof(b200_block), 256);
   const size_t mv_bytes = mv_src ? b200_align_up(nblocks * sizeof(b200_me_result), 256) : 0;
-  B200_CUDA(ctx, cudaSetDevice(ctx->device));
-  void *dbase = nullptr;
-  B200_CUDA(ctx, cudaMallocAsync(&dbase, blk_bytes + mv_bytes + out_bytes, ctx->stream));
-  uint8_t *d_blk = (uint8_t *)dbase, *d_mv = d_blk + blk_bytes, *d_out = d_mv + mv_bytes;
-  int st = B200_OK;
-  if (cudaMemcpyAsync(d_blk, blocks, nblocks * sizeof(b200_block), cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess ||
-      (mv_src && cudaMemcpyAsync(d_mv, mv_src, nblocks * sizeof(b200_me_result), cudaMemcpyHostToDevice,
-                                 ctx->stream) != cudaSuccess))
-    st = b200_fail(ctx, B200_ERR_CUDA, "H2D copy failed");
-  if (!st)
-    st = b200_fwd_txfm_residual_dev(ctx, cur, ref, (const b200_block *)d_blk, nblocks,
-                                    mv_src ? (const b200_me_result *)d_mv : nullptr, d_out, tx_size,
-                                    tx_type, bd);
-  if (!st && cudaMemcpyAsync(output, d_out, out_bytes, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess)
-    st = b200_fail(ctx, B200_ERR_CUDA, "D2H copy failed");
-  cudaFreeAsync(dbase, ctx->stream);
-  if (st) return st;
-  if (!ctx->async_batch) B200_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  return B200_OK;
+  HostStage s(ctx, blk_bytes + mv_bytes + out_bytes);
+  b200_block *d_blk = (b200_block *)s.take(nblocks * sizeof(b200_block));
+  b200_me_result *d_mv = mv_src ? (b200_me_result *)s.take(nblocks * sizeof(b200_me_result)) : nullptr;
+  uint8_t *d_out = s.take(out_bytes);
+  s.up(d_blk, blocks, nblocks * sizeof(b200_block));
+  if (mv_src) s.up(d_mv, mv_src, nblocks * sizeof(b200_me_result));
+  if (s.ok()) s.run(b200_fwd_txfm_residual_dev(ctx, cur, ref, d_blk, nblocks, d_mv, d_out, tx_size, tx_type, bd));
+  s.down(output, d_out, out_bytes);
+  return s.finish(!ctx->async_batch);
 }
 
 // Per-call form with the reference's signature (asm/x86/transform/forward.rs:444-447):
@@ -380,9 +363,7 @@ extern "C" int b200_fwd_txfm_residual_resident(b200_ctx *ctx, const b200_plane *
 extern "C" void b200_forward_transform(const int16_t *input, void *output, size_t stride,
                                        int tx_size, int tx_type, int bd, int coeff_is_i32) {
   b200_ctx *ctx = b200_default_ctx();
-  int st = b200_fwd_txfm_batch(ctx, input, 0, stride, output, 1, tx_size, tx_type, bd, coeff_is_i32);
-  if (st != B200_OK) {
-    fprintf(stderr, "b200rdo: FATAL: forward_transform failed: %s\n", b200_last_error(ctx));
-    abort();  // the reference panics on an invalid (size, type) pair (forward.rs:75)
-  }
+  // the reference panics on an invalid (size, type) pair (forward.rs:75)
+  b200_percall_check(ctx, b200_fwd_txfm_batch(ctx, input, 0, stride, output, 1, tx_size, tx_type, bd, coeff_is_i32),
+                     "forward_transform");
 }

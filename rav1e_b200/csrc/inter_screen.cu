@@ -20,7 +20,6 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
-#include <mutex>
 
 #include "common.cuh"
 #include "mc_dev.cuh"
@@ -244,12 +243,7 @@ int launch_class(b200_ctx *ctx, ScreenArgs a) {
   constexpr int S = 16 << CLS;
   const size_t per_warp = ScreenLayout<T, S>::BYTES;
   const int wpc = (int)std::min<size_t>(kMaxWarps, std::max<size_t>(1, (200 * 1024) / per_warp));
-  static std::once_flag once;
-  static cudaError_t err = cudaSuccess;
-  std::call_once(once, [] {
-    err = cudaFuncSetAttribute(inter_screen_kernel<T, CLS>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-  });
-  B200_CUDA(ctx, err);
+  if (int st = b200_smem_opt_in(ctx, (const void *)inter_screen_kernel<T, CLS>, 200 * 1024)) return st;
   a.smem_per_warp = (int)per_warp;
   // the class's item count lives on the device: enough warps for every item up to a few waves
   const int grid = (int)std::min<size_t>((a.n + wpc - 1) / wpc, (size_t)ctx->num_sms * 8);

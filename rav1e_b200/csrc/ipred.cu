@@ -5,7 +5,7 @@
 // small IntraEdge buffer (partition.rs:600-637) and write a packed w x h prediction.  The
 // edge buffer is staged in shared memory, the CTA runs the preparation step of ipred_dev.cuh
 // (DC value, edge filter and upsampler) and then every thread evaluates its pixels.
-#include "common.cuh"
+#include "host_stage.cuh"
 #include "ipred_dev.cuh"
 
 namespace {
@@ -165,13 +165,9 @@ extern "C" void b200_predict_intra(int mode, int variant, void *dst, ptrdiff_t d
   const int bpp = bit_depth == 8 ? 1 : 2;
   const size_t edge_bytes = b200_align_up((size_t)kEdgeLen * bpp, 256);
   const size_t ac_bytes = b200_align_up((size_t)w * h * 2, 256);
-  void *dbase = nullptr;
-  int st = B200_OK;
-  if (cudaSetDevice(ctx->device) != cudaSuccess ||
-      cudaMallocAsync(&dbase, edge_bytes + ac_bytes + 256 + (size_t)w * h * bpp, ctx->stream) != cudaSuccess)
-    st = b200_fail(ctx, B200_ERR_CUDA, "alloc failed");
-  uint8_t *d_edge = (uint8_t *)dbase, *d_ac = d_edge + edge_bytes, *d_item = d_ac + ac_bytes,
-          *d_out = d_item + 256;
+  HostStage s(ctx, edge_bytes + ac_bytes + 256 + (size_t)w * h * bpp);
+  uint8_t *d_edge = s.take((size_t)kEdgeLen * bpp), *d_ac = s.take((size_t)w * h * 2);
+  uint8_t *d_item = s.take(sizeof(b200_intra_item)), *d_out = s.take((size_t)w * h * bpp);
   b200_intra_item item{};
   item.edge = 0;
   item.ac = 0;
@@ -183,20 +179,12 @@ extern "C" void b200_predict_intra(int mode, int variant, void *dst, ptrdiff_t d
   item.ief = (int8_t)ief;
   item.left_len = (uint8_t)left_len;
   item.above_len = (uint8_t)above_len;
-  if (!st && (cudaMemcpyAsync(d_edge, edge, (size_t)kEdgeLen * bpp, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess ||
-              cudaMemcpyAsync(d_item, &item, sizeof item, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess ||
-              (ac && cudaMemcpyAsync(d_ac, ac, (size_t)w * h * 2, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess)))
-    st = b200_fail(ctx, B200_ERR_CUDA, "H2D copy failed");
-  if (!st)
-    st = b200_predict_intra_dev(ctx, d_edge, (const b200_intra_item *)d_item, 1, (const int16_t *)d_ac, w, h,
-                                bit_depth, plane_w, plane_h, d_out);
-  if (!st && cudaMemcpy2DAsync(dst, (size_t)dst_stride, d_out, (size_t)w * bpp, (size_t)w * bpp, h,
-                               cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess)
-    st = b200_fail(ctx, B200_ERR_CUDA, "D2H copy failed");
-  if (dbase) cudaFreeAsync(dbase, ctx->stream);
-  if (!st && cudaStreamSynchronize(ctx->stream) != cudaSuccess) st = b200_fail(ctx, B200_ERR_CUDA, "sync failed");
-  if (st) {
-    fprintf(stderr, "b200rdo: FATAL: predict_intra failed: %s\n", b200_last_error(ctx));
-    abort();
-  }
+  s.up(d_edge, edge, (size_t)kEdgeLen * bpp);
+  s.up(d_item, &item, sizeof item);
+  if (ac) s.up(d_ac, ac, (size_t)w * h * 2);
+  if (s.ok())
+    s.run(b200_predict_intra_dev(ctx, d_edge, (const b200_intra_item *)d_item, 1, (const int16_t *)d_ac, w, h,
+                                 bit_depth, plane_w, plane_h, d_out));
+  s.down2d(dst, (size_t)dst_stride, d_out, (size_t)w * bpp, (size_t)w * bpp, h);
+  b200_percall_check(ctx, s.finish(true), "predict_intra");
 }

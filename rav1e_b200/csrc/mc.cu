@@ -7,8 +7,7 @@
 // `prep` writes the biased i16 intermediate used by compound prediction, `avg` blends two of
 // those (mc.rs:454-479).  Blocks are addressed by (position, motion vector) through
 // get_mv_params (predict.rs:284-297), so one launch predicts thousands of blocks.
-#include <mutex>
-
+#include "host_stage.cuh"
 #include "mc_dev.cuh"
 
 namespace {
@@ -185,12 +184,7 @@ int launch_mc_fast(b200_ctx *ctx, const McArgs &a) {
   using ML = McLayout<T, N, N>;
   const size_t per_warp = b200_align_up(ML::TILE_BYTES + ML::INTER_BYTES, 16);
   const int wpc = (int)std::min<size_t>(8, std::max<size_t>(1, (128 * 1024) / per_warp));
-  static std::once_flag once;
-  static cudaError_t err = cudaSuccess;
-  std::call_once(once, [] {
-    err = cudaFuncSetAttribute(mc_put_fast_kernel<T, N, N>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
-  });
-  B200_CUDA(ctx, err);
+  if (int st = b200_smem_opt_in(ctx, (const void *)mc_put_fast_kernel<T, N, N>, 160 * 1024)) return st;
   const int grid = (int)std::min<size_t>((a.n + wpc - 1) / wpc, (size_t)ctx->num_sms * 16);
   mc_put_fast_kernel<T, N, N><<<grid, wpc * 32, per_warp * wpc, ctx->stream>>>(a, (int)per_warp);
   B200_LAUNCH_CHECK(ctx);
@@ -221,14 +215,10 @@ int launch_mc(b200_ctx *ctx, const McArgs &a, int bpp) {
   // warps (= blocks in flight) per CTA: as many as fit ~96 KB, at most 8
   int wpc = (int)std::min<size_t>(8, std::max<size_t>(1, (96 * 1024) / per_warp));
   const size_t smem = per_warp * wpc;
-  static std::once_flag attr_once;
-  static cudaError_t attr_err = cudaSuccess;
-  std::call_once(attr_once, [] {  // thread safe; 128 KB covers one 128x128 u16 block per warp slot
-    attr_err = cudaFuncSetAttribute(mc_kernel<uint8_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024);
-    if (attr_err == cudaSuccess)
-      attr_err = cudaFuncSetAttribute(mc_kernel<uint16_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024);
-  });
-  B200_CUDA(ctx, attr_err);
+  // 128 KB covers one 128x128 u16 block per warp slot
+  if (int st = b200_smem_opt_in(ctx, bpp == 1 ? (const void *)mc_kernel<uint8_t> : (const void *)mc_kernel<uint16_t>,
+                                128 * 1024))
+    return st;
   const size_t ctas = (a.n + wpc - 1) / wpc;
   const int grid = (int)std::min<size_t>(ctas, (size_t)ctx->num_sms * 16);
   if (bpp == 1)
@@ -321,18 +311,13 @@ int percall_mc(int kind, void *dst, ptrdiff_t dst_stride, const void *src, ptrdi
   B200_REQUIRE(ctx, col_frac >= 0 && col_frac < 16 && row_frac >= 0 && row_frac < 16, "bad fraction");
   const int bpp = bit_depth == 8 ? 1 : 2;
   const int tw = w + 7, th = h + 7;
-  const size_t tile_bytes = b200_align_up((size_t)tw * th * bpp, 256);
   const size_t out_bytes = (size_t)w * h * (kind == 0 ? bpp : 2);
-  void *dbase = nullptr;
-  B200_CUDA(ctx, cudaSetDevice(ctx->device));
-  B200_CUDA(ctx, cudaMallocAsync(&dbase, tile_bytes + out_bytes, ctx->stream));
+  HostStage s(ctx, b200_align_up((size_t)tw * th * bpp, 256) + out_bytes);
+  uint8_t *d_tile = s.take((size_t)tw * th * bpp);
   const uint8_t *h0 = (const uint8_t *)src - 3 * src_stride - 3 * bpp;  // asm/x86/mc.rs:122-123
-  int st = B200_OK;
-  if (cudaMemcpy2DAsync(dbase, (size_t)tw * bpp, h0, (size_t)src_stride, (size_t)tw * bpp, th,
-                        cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess)
-    st = b200_fail(ctx, B200_ERR_CUDA, "H2D copy failed");
+  s.up2d(d_tile, (size_t)tw * bpp, h0, (size_t)src_stride, (size_t)tw * bpp, th);
   McArgs a{};
-  a.ref = (uint8_t *)dbase + ((size_t)3 * tw + 3) * bpp;
+  a.ref = d_tile + ((size_t)3 * tw + 3) * bpp;
   a.ref_stride = tw;
   a.n = 1;
   a.w = w;
@@ -341,45 +326,31 @@ int percall_mc(int kind, void *dst, ptrdiff_t dst_stride, const void *src, ptrdi
   a.mode_y = mode_y;
   a.bit_depth = bit_depth;
   a.kind = kind;
-  a.out = (uint8_t *)dbase + tile_bytes;
+  a.out = s.take(out_bytes);
   a.explicit_frac = 1;
   a.col_frac = col_frac;
   a.row_frac = row_frac;
-  if (!st) st = launch_mc(ctx, a, bpp);
-  if (!st) {
-    cudaError_t e;
-    if (kind == 0)
-      e = cudaMemcpy2DAsync(dst, (size_t)dst_stride, a.out, (size_t)w * bpp, (size_t)w * bpp, h,
-                            cudaMemcpyDeviceToHost, ctx->stream);
-    else
-      e = cudaMemcpyAsync(dst, a.out, out_bytes, cudaMemcpyDeviceToHost, ctx->stream);
-    if (e != cudaSuccess) st = b200_fail(ctx, B200_ERR_CUDA, "D2H copy failed");
-  }
-  cudaFreeAsync(dbase, ctx->stream);
-  if (st) return st;
-  B200_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  return B200_OK;
-}
-void die_if(int st, const char *what) {
-  if (st != B200_OK) {
-    fprintf(stderr, "b200rdo: FATAL: %s failed: %s\n", what, b200_last_error(b200_default_ctx()));
-    abort();  // the reference asserts (mc.rs:256-257) and has no error return
-  }
+  if (s.ok()) s.run(launch_mc(ctx, a, bpp));
+  if (kind == 0)
+    s.down2d(dst, (size_t)dst_stride, a.out, (size_t)w * bpp, (size_t)w * bpp, h);
+  else
+    s.down(dst, a.out, out_bytes);
+  return s.finish(true);
 }
 }  // namespace
 
 extern "C" void b200_put_8tap(void *dst, ptrdiff_t dst_stride, const void *src, ptrdiff_t src_stride,
                               int w, int h, int col_frac, int row_frac, int mode_x, int mode_y,
                               int bit_depth) {
-  die_if(percall_mc(0, dst, dst_stride, src, src_stride, w, h, col_frac, row_frac, mode_x, mode_y,
-                    bit_depth),
-         "put_8tap");
+  // the reference asserts (mc.rs:256-257) and has no error return
+  const int st = percall_mc(0, dst, dst_stride, src, src_stride, w, h, col_frac, row_frac, mode_x, mode_y, bit_depth);
+  b200_percall_check(b200_default_ctx(), st, "put_8tap");
 }
 
 extern "C" void b200_prep_8tap(int16_t *tmp, const void *src, ptrdiff_t src_stride, int w, int h,
                                int col_frac, int row_frac, int mode_x, int mode_y, int bit_depth) {
-  die_if(percall_mc(1, tmp, 0, src, src_stride, w, h, col_frac, row_frac, mode_x, mode_y, bit_depth),
-         "prep_8tap");
+  const int st = percall_mc(1, tmp, 0, src, src_stride, w, h, col_frac, row_frac, mode_x, mode_y, bit_depth);
+  b200_percall_check(b200_default_ctx(), st, "prep_8tap");
 }
 
 extern "C" void b200_mc_avg(void *dst, ptrdiff_t dst_stride, const int16_t *tmp1, const int16_t *tmp2,
@@ -387,21 +358,12 @@ extern "C" void b200_mc_avg(void *dst, ptrdiff_t dst_stride, const int16_t *tmp1
   b200_ctx *ctx = b200_default_ctx();
   const int bpp = bit_depth == 8 ? 1 : 2;
   const size_t n = (size_t)w * h;
-  void *dbase = nullptr;
-  int st = B200_OK;
-  if (cudaSetDevice(ctx->device) != cudaSuccess ||
-      cudaMallocAsync(&dbase, n * 4 + n * bpp + 512, ctx->stream) != cudaSuccess)
-    st = b200_fail(ctx, B200_ERR_CUDA, "alloc failed");
-  int16_t *d1 = (int16_t *)dbase, *d2 = d1 + n;
-  uint8_t *dd = (uint8_t *)(d2 + n);
-  if (!st && (cudaMemcpyAsync(d1, tmp1, n * 2, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess ||
-              cudaMemcpyAsync(d2, tmp2, n * 2, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess))
-    st = b200_fail(ctx, B200_ERR_CUDA, "H2D copy failed");
-  if (!st) st = b200_mc_avg_dev(ctx, d1, d2, dd, 1, w, h, bit_depth);
-  if (!st && cudaMemcpy2DAsync(dst, (size_t)dst_stride, dd, (size_t)w * bpp, (size_t)w * bpp, h,
-                               cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess)
-    st = b200_fail(ctx, B200_ERR_CUDA, "D2H copy failed");
-  if (dbase) cudaFreeAsync(dbase, ctx->stream);
-  if (!st && cudaStreamSynchronize(ctx->stream) != cudaSuccess) st = b200_fail(ctx, B200_ERR_CUDA, "sync failed");
-  die_if(st, "mc_avg");
+  HostStage s(ctx, n * 4 + n * bpp + 512);
+  int16_t *d1 = (int16_t *)s.take(n * 2), *d2 = (int16_t *)s.take(n * 2);
+  uint8_t *dd = s.take(n * bpp);
+  s.up(d1, tmp1, n * 2);
+  s.up(d2, tmp2, n * 2);
+  if (s.ok()) s.run(b200_mc_avg_dev(ctx, d1, d2, dd, 1, w, h, bit_depth));
+  s.down2d(dst, (size_t)dst_stride, dd, (size_t)w * bpp, (size_t)w * bpp, h);
+  b200_percall_check(ctx, s.finish(true), "mc_avg");
 }

@@ -961,15 +961,8 @@ bool chunk_lists_ok(const MeArgs &a) {
 
 template <int W, int H, bool SATD>
 int launch_cand_group(b200_ctx *ctx, MeArgs a, int window_hint_px, const b200_plane *refs) {
-  // opt in to the largest dynamic shared memory this kernel may be launched with, once
-  // (thread safe: contexts on several host threads launch concurrently)
-  static std::once_flag attr_once;
-  static cudaError_t attr_err = cudaSuccess;
-  std::call_once(attr_once, [] {
-    attr_err = cudaFuncSetAttribute(me_cand_group_u8<W, H, SATD>,
-                                    cudaFuncAttributeMaxDynamicSharedMemorySize, kCandSmemBytes);
-  });
-  B200_CUDA(ctx, attr_err);
+  // opt in to the largest dynamic shared memory this kernel may be launched with
+  if (int st = b200_smem_opt_in(ctx, (const void *)me_cand_group_u8<W, H, SATD>, kCandSmemBytes)) return st;
   bool cur_word_pitch = true;
   for (int k = 0; k < a.pr.n; k++) cur_word_pitch = cur_word_pitch && (a.pr.cur[k].stride & 3) == 0;
   {

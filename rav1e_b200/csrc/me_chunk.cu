@@ -28,8 +28,6 @@
 // one final rounding.
 #include <cuda_runtime.h>
 
-#include <mutex>
-
 #include "common.cuh"
 #include "me_cand.cuh"
 #include "me_dev.cuh"
@@ -369,12 +367,7 @@ __global__ void __launch_bounds__(256, B200_SATD_SPARSE_MINBLOCKS)
 template <typename T, int W, int H, bool SATD>
 int launch_chunk_lists(b200_ctx *ctx, const MeArgs &a) {
   using C = SatdSparseCfg<T, W, H>;
-  static std::once_flag once;
-  static cudaError_t err = cudaSuccess;
-  std::call_once(once, [] {
-    err = cudaFuncSetAttribute(me_chunk_lists<T, W, H, SATD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM);
-  });
-  B200_CUDA(ctx, err);
+  if (int st = b200_smem_opt_in(ctx, (const void *)me_chunk_lists<T, W, H, SATD>, (int)C::SMEM)) return st;
   const int wpc = C::WARPS;
   const int grid = (int)std::min<size_t>((a.nblocks + wpc - 1) / wpc, (size_t)ctx->num_sms * 16);
   me_chunk_lists<T, W, H, SATD><<<grid, wpc * 32, C::SMEM, ctx->stream>>>(a);

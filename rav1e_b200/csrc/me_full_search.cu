@@ -9,7 +9,6 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
-#include <mutex>
 
 #include "common.cuh"
 #include "me_dev.cuh"
@@ -204,13 +203,7 @@ __global__ void __launch_bounds__(256) me_full_search_u8(FsArgs a) {
 template <int W, int H>
 int launch_fs_u8(b200_ctx *ctx, const FsArgs &a, size_t smem_bytes) {
   constexpr int NP = W >= 8 ? 4 : 2;
-  static std::once_flag attr_once;
-  static cudaError_t attr_err = cudaSuccess;
-  std::call_once(attr_once, [] {
-    attr_err = cudaFuncSetAttribute(me_full_search_u8<W, H, NP>,
-                                    cudaFuncAttributeMaxDynamicSharedMemorySize, kFsSmemBytes);
-  });
-  B200_CUDA(ctx, attr_err);
+  if (int st = b200_smem_opt_in(ctx, (const void *)me_full_search_u8<W, H, NP>, kFsSmemBytes)) return st;
   const int grid = (int)std::min<size_t>(a.nblocks, (size_t)ctx->num_sms * 32);
   me_full_search_u8<W, H, NP><<<grid, 256, smem_bytes, ctx->stream>>>(a);
   B200_LAUNCH_CHECK(ctx);

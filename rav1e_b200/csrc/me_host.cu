@@ -1,7 +1,7 @@
 // me_host.cu — host-buffer (`*_batch`) and per-call reference-signature entry points of the
 // SAD/SATD/ME path.  They copy the caller's host buffers (pinned or pageable) to a stream-
 // ordered device allocation, run the same device kernels as the `_dev` forms (me_cand.cu, me_full_search.cu) and copy results back before returning.
-#include "common.cuh"
+#include "host_stage.cuh"
 
 namespace {
 
@@ -17,16 +17,14 @@ size_t staged_pitch(const b200_host_plane *hp) {
   return b200_align_up(staged_lead(hp) + (size_t)(hp->width + hp->pad) * hp->bpp + 64, 128);
 }
 
-int upload_host_plane(b200_ctx *ctx, const b200_host_plane *hp, uint8_t *dbase, b200_plane *out) {
+void upload_host_plane(HostStage &s, const b200_host_plane *hp, uint8_t *dbase, b200_plane *out) {
   const size_t pitch = staged_pitch(hp);
   size_t row_bytes, rows;
   host_plane_span(hp, &row_bytes, &rows);
   const uint8_t *h0 = (const uint8_t *)hp->data - (ptrdiff_t)hp->pad * hp->stride -
                       (ptrdiff_t)hp->pad * hp->bpp;
   const size_t lead = staged_lead(hp);
-  B200_CUDA(ctx, cudaMemcpy2DAsync(dbase + lead - (size_t)hp->pad * hp->bpp, pitch, h0,
-                                   (size_t)hp->stride, row_bytes, rows, cudaMemcpyHostToDevice,
-                                   ctx->stream));
+  s.up2d(dbase + lead - (size_t)hp->pad * hp->bpp, pitch, h0, (size_t)hp->stride, row_bytes, rows);
   out->alloc = nullptr;
   out->data = dbase + (size_t)hp->pad * pitch + lead;
   out->stride = (int32_t)(pitch / hp->bpp);
@@ -34,7 +32,6 @@ int upload_host_plane(b200_ctx *ctx, const b200_host_plane *hp, uint8_t *dbase, 
   out->height = hp->height;
   out->pad = hp->pad;
   out->bpp = hp->bpp;
-  return B200_OK;
 }
 
 int check_host_plane(b200_ctx *ctx, const b200_host_plane *hp) {
@@ -45,17 +42,6 @@ int check_host_plane(b200_ctx *ctx, const b200_host_plane *hp) {
                "host stride smaller than width + 2*pad");
   return B200_OK;
 }
-
-struct Carver {
-  uint8_t *p;
-  size_t used = 0;
-  explicit Carver(void *base) : p((uint8_t *)base) {}
-  uint8_t *take(size_t bytes) {
-    uint8_t *r = p + used;
-    used += b200_align_up(bytes, 256);
-    return r;
-  }
-};
 
 }  // namespace
 
@@ -95,8 +81,6 @@ static int me_candidates_host_impl(b200_ctx *ctx, const b200_host_plane *cur,
   B200_REQUIRE(ctx, params && blocks && (cands || mvs || !ncands), "NULL params/blocks/cands");
   B200_REQUIRE(ctx, !mvs || cand_offsets, "MotionVector lists need cand_offsets (the CSR names the block)");
   B200_REQUIRE(ctx, best == nullptr || cand_offsets != nullptr, "best needs cand_offsets");
-  B200_CUDA(ctx, cudaSetDevice(ctx->device));
-
   size_t rb, rows;
   const size_t cur_bytes = rcur ? 0 : staged_pitch(cur) * (host_plane_span(cur, &rb, &rows), rows) + 512;
   const size_t ref_bytes = rcur ? 0 : staged_pitch(ref) * (host_plane_span(ref, &rb, &rows), rows) + 512;
@@ -106,65 +90,43 @@ static int me_candidates_host_impl(b200_ctx *ctx, const b200_host_plane *cur,
                  (best ? nblocks * sizeof(b200_me_result) : 0) + (mvs ? ncands * 4 : 0) + 16 * 256;
   // leave room for the generic path's internal cost/sad scratch (b200_reserve_dwork is
   // grow-only and shared): carve our buffers from a private allocation instead.
-  void *dbase = nullptr;
-  B200_CUDA(ctx, cudaMallocAsync(&dbase, total, ctx->stream));
-  Carver c(dbase);
+  HostStage s(ctx, total);
   b200_plane dcur, dref;
-  int st = B200_OK;
   if (rcur) {
     dcur = *rcur;
     dref = *rref;
   } else {
-    st = upload_host_plane(ctx, cur, c.take(cur_bytes), &dcur);
-    if (!st) st = upload_host_plane(ctx, ref, c.take(ref_bytes), &dref);
+    upload_host_plane(s, cur, s.take(cur_bytes), &dcur);
+    upload_host_plane(s, ref, s.take(ref_bytes), &dref);
   }
-  b200_block *d_blocks = (b200_block *)c.take(nblocks * sizeof(b200_block));
-  b200_cand *d_cands = (b200_cand *)c.take(ncands * sizeof(b200_cand));
-  short2 *d_mvs = mvs ? (short2 *)c.take(ncands * 4) : nullptr;
-  uint32_t *d_offs = cand_offsets ? (uint32_t *)c.take((nblocks + 1) * 4) : nullptr;
-  int16_t *d_pmv = pmv ? (int16_t *)c.take(nblocks * 8) : nullptr;
-  uint32_t *d_sad = sad ? (uint32_t *)c.take(ncands * 4) : nullptr;
-  uint64_t *d_cost = cost ? (uint64_t *)c.take(ncands * 8) : nullptr;
-  b200_me_result *d_best = best ? (b200_me_result *)c.take(nblocks * sizeof(b200_me_result)) : nullptr;
-  auto fail = [&](int s) {
-    cudaFreeAsync(dbase, ctx->stream);
-    return s;
-  };
-  if (st) return fail(st);
-#define H2D(dst, src, bytes)                                                                   \
-  if ((bytes) != 0 && cudaMemcpyAsync((dst), (src), (bytes), cudaMemcpyHostToDevice, ctx->stream) != \
-                     cudaSuccess)                                                              \
-    return fail(b200_fail(ctx, B200_ERR_CUDA, "H2D copy failed: %s",                           \
-                          cudaGetErrorString(cudaGetLastError())));
-  H2D(d_blocks, blocks, nblocks * sizeof(b200_block));
+  b200_block *d_blocks = (b200_block *)s.take(nblocks * sizeof(b200_block));
+  b200_cand *d_cands = (b200_cand *)s.take(ncands * sizeof(b200_cand));
+  short2 *d_mvs = mvs ? (short2 *)s.take(ncands * 4) : nullptr;
+  uint32_t *d_offs = cand_offsets ? (uint32_t *)s.take((nblocks + 1) * 4) : nullptr;
+  int16_t *d_pmv = pmv ? (int16_t *)s.take(nblocks * 8) : nullptr;
+  uint32_t *d_sad = sad ? (uint32_t *)s.take(ncands * 4) : nullptr;
+  uint64_t *d_cost = cost ? (uint64_t *)s.take(ncands * 8) : nullptr;
+  b200_me_result *d_best = best ? (b200_me_result *)s.take(nblocks * sizeof(b200_me_result)) : nullptr;
+  s.up(d_blocks, blocks, nblocks * sizeof(b200_block));
   if (d_mvs) {
-    H2D(d_mvs, mvs, ncands * 4);
+    s.up(d_mvs, mvs, ncands * 4);
   } else {
-    H2D(d_cands, cands, ncands * sizeof(b200_cand));
+    s.up(d_cands, cands, ncands * sizeof(b200_cand));
   }
-  if (d_offs) H2D(d_offs, cand_offsets, (nblocks + 1) * 4);
-  if (d_mvs && ncands) {
+  if (d_offs) s.up(d_offs, cand_offsets, (nblocks + 1) * 4);
+  if (s.ok() && d_mvs && ncands) {
     const int grid = (int)std::min<size_t>((nblocks + 7) / 8, (size_t)ctx->num_sms * 16);
     expand_mvs_kernel<<<grid, 256, 0, ctx->stream>>>(d_mvs, d_offs, nblocks, d_cands);
     ctx->launches++;
   }
-  if (d_pmv) H2D(d_pmv, pmv, nblocks * 8);
-#undef H2D
-  st = b200_me_candidates_dev(ctx, &dcur, &dref, d_blocks, nblocks, d_cands, ncands, d_offs, d_pmv,
-                              params, d_sad, d_cost, d_best);
-  if (st) return fail(st);
-#define D2H(dst, src, bytes)                                                                   \
-  if ((bytes) != 0 && cudaMemcpyAsync((dst), (src), (bytes), cudaMemcpyDeviceToHost, ctx->stream) != \
-                     cudaSuccess)                                                              \
-    return fail(b200_fail(ctx, B200_ERR_CUDA, "D2H copy failed: %s",                           \
-                          cudaGetErrorString(cudaGetLastError())));
-  if (sad) D2H(sad, d_sad, ncands * 4);
-  if (cost) D2H(cost, d_cost, ncands * 8);
-  if (best) D2H(best, d_best, nblocks * sizeof(b200_me_result));
-#undef D2H
-  cudaFreeAsync(dbase, ctx->stream);
-  if (!ctx->async_batch) B200_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  return B200_OK;
+  if (d_pmv) s.up(d_pmv, pmv, nblocks * 8);
+  if (s.ok())
+    s.run(b200_me_candidates_dev(ctx, &dcur, &dref, d_blocks, nblocks, d_cands, ncands, d_offs, d_pmv, params,
+                                 d_sad, d_cost, d_best));
+  if (sad) s.down(sad, d_sad, ncands * 4);
+  if (cost) s.down(cost, d_cost, ncands * 8);
+  if (best) s.down(best, d_best, nblocks * sizeof(b200_me_result));
+  return s.finish(!ctx->async_batch);
 }
 
 extern "C" int b200_me_candidates_batch(b200_ctx *ctx, const b200_host_plane *cur,
@@ -209,32 +171,20 @@ extern "C" int b200_me_full_search_batch(b200_ctx *ctx, const b200_host_plane *c
   if (int st = check_host_plane(ctx, cur)) return st;
   if (int st = check_host_plane(ctx, ref)) return st;
   B200_REQUIRE(ctx, params && blocks && best, "NULL params/blocks/best");
-  B200_CUDA(ctx, cudaSetDevice(ctx->device));
   size_t rb, rows;
   const size_t cur_bytes = staged_pitch(cur) * (host_plane_span(cur, &rb, &rows), rows) + 512;
   const size_t ref_bytes = staged_pitch(ref) * (host_plane_span(ref, &rb, &rows), rows) + 512;
-  const size_t total = cur_bytes + ref_bytes + nblocks * (sizeof(b200_block) + sizeof(b200_me_result)) + 8 * 256;
-  void *dbase = nullptr;
-  B200_CUDA(ctx, cudaMallocAsync(&dbase, total, ctx->stream));
-  Carver c(dbase);
+  HostStage s(ctx, cur_bytes + ref_bytes + nblocks * (sizeof(b200_block) + sizeof(b200_me_result)) + 8 * 256);
   b200_plane dcur, dref;
-  int st = upload_host_plane(ctx, cur, c.take(cur_bytes), &dcur);
-  if (!st) st = upload_host_plane(ctx, ref, c.take(ref_bytes), &dref);
-  b200_block *d_blocks = (b200_block *)c.take(nblocks * sizeof(b200_block));
-  b200_me_result *d_best = (b200_me_result *)c.take(nblocks * sizeof(b200_me_result));
-  if (!st && cudaMemcpyAsync(d_blocks, blocks, nblocks * sizeof(b200_block), cudaMemcpyHostToDevice,
-                             ctx->stream) != cudaSuccess)
-    st = b200_fail(ctx, B200_ERR_CUDA, "H2D copy failed");
-  if (!st)
-    st = b200_me_full_search_dev(ctx, &dcur, &dref, d_blocks, nblocks, params, range_x, range_y,
-                                 step, d_best);
-  if (!st && cudaMemcpyAsync(best, d_best, nblocks * sizeof(b200_me_result), cudaMemcpyDeviceToHost,
-                             ctx->stream) != cudaSuccess)
-    st = b200_fail(ctx, B200_ERR_CUDA, "D2H copy failed");
-  cudaFreeAsync(dbase, ctx->stream);
-  if (st) return st;
-  B200_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  return B200_OK;
+  upload_host_plane(s, cur, s.take(cur_bytes), &dcur);
+  upload_host_plane(s, ref, s.take(ref_bytes), &dref);
+  b200_block *d_blocks = (b200_block *)s.take(nblocks * sizeof(b200_block));
+  b200_me_result *d_best = (b200_me_result *)s.take(nblocks * sizeof(b200_me_result));
+  s.up(d_blocks, blocks, nblocks * sizeof(b200_block));
+  if (s.ok())
+    s.run(b200_me_full_search_dev(ctx, &dcur, &dref, d_blocks, nblocks, params, range_x, range_y, step, d_best));
+  s.down(best, d_best, nblocks * sizeof(b200_me_result));
+  return s.finish(true);
 }
 
 // ------------------------------------------------------------------ per-call forms
@@ -258,12 +208,10 @@ uint32_t percall_dist(const void *org, ptrdiff_t org_stride, const void *ref, pt
   p.use_satd = use_satd;
   p.bit_depth = bpp == 1 ? 8 : 10;
   uint32_t out = 0;
-  int st = b200_me_candidates_batch(ctx, &hc, &hr, &blk, 1, &cand, 1, nullptr, nullptr, &p, &out,
-                                    nullptr, nullptr);
-  if (st != B200_OK) {
-    fprintf(stderr, "b200rdo: FATAL: per-call distortion failed: %s\n", b200_last_error(ctx));
-    abort();  // the reference has no error return here either; never silently wrong
-  }
+  b200_percall_check(ctx,
+                     b200_me_candidates_batch(ctx, &hc, &hr, &blk, 1, &cand, 1, nullptr, nullptr, &p, &out, nullptr,
+                                              nullptr),
+                     "per-call distortion");
   return out;
 }
 

@@ -14,7 +14,7 @@
 
 #include <algorithm>
 
-#include "common.cuh"
+#include "host_stage.cuh"
 
 namespace {
 
@@ -84,20 +84,14 @@ extern "C" double b200_compute_rd_cost(double lambda, uint32_t rate, uint64_t di
     unsigned long long dist;
     double cost;
     uint32_t rate;
-  } h{distortion, 0.0, rate}, *d = nullptr;
-  int st = B200_OK;
-  if (cudaSetDevice(ctx->device) != cudaSuccess || cudaMallocAsync((void **)&d, sizeof h, ctx->stream) != cudaSuccess)
-    st = b200_fail(ctx, B200_ERR_CUDA, "alloc failed");
-  if (!st && cudaMemcpyAsync(d, &h, sizeof h, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess)
-    st = b200_fail(ctx, B200_ERR_CUDA, "H2D copy failed");
-  if (!st) st = b200_compute_rd_cost_dev(ctx, lambda, &d->rate, (const uint64_t *)&d->dist, 1, nullptr, 0, &d->cost, nullptr);
-  if (!st && cudaMemcpyAsync(&h.cost, &d->cost, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess)
-    st = b200_fail(ctx, B200_ERR_CUDA, "D2H copy failed");
-  if (d) cudaFreeAsync(d, ctx->stream);
-  if (!st && cudaStreamSynchronize(ctx->stream) != cudaSuccess) st = b200_fail(ctx, B200_ERR_CUDA, "sync failed");
-  if (st) {
-    fprintf(stderr, "b200rdo: FATAL: compute_rd_cost failed: %s\n", b200_last_error(ctx));
-    abort();
-  }
+  } h{distortion, 0.0, rate};
+  HostStage s(ctx, sizeof h);
+  auto *d = (decltype(h) *)s.take(sizeof h);
+  s.up(d, &h, sizeof h);
+  if (s.ok())
+    s.run(b200_compute_rd_cost_dev(ctx, lambda, &d->rate, (const uint64_t *)&d->dist, 1, nullptr, 0, &d->cost,
+                                   nullptr));
+  s.down(&h.cost, &d->cost, sizeof(double));
+  b200_percall_check(ctx, s.finish(true), "compute_rd_cost");
   return h.cost;
 }

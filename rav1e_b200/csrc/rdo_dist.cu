@@ -15,6 +15,7 @@
 #include <algorithm>
 #include <mutex>
 
+#include "host_stage.cuh"
 #include "rdo_dist_dev.cuh"
 
 namespace {
@@ -91,30 +92,19 @@ int check_pair(b200_ctx *ctx, const b200_plane *a, const b200_plane *b) {
 }
 
 
-// stage two host blocks (w x h, byte strides) into a scratch device plane pair
-struct HostPair {
-  void *dbase = nullptr;
-  b200_plane a{}, b{};
-};
+// A host block (w x h, byte stride) staged as a device plane with a 16-byte row pitch.
+size_t staged_block_bytes(int w, int h, int bpp) { return b200_align_up((size_t)w * bpp, 16) * h; }
 
-int stage_pair(b200_ctx *ctx, const void *src, ptrdiff_t ss, const void *dst, ptrdiff_t ds, int w, int h,
-               int bpp, size_t extra, HostPair *hp, uint8_t **extra_ptr) {
+b200_plane stage_block(HostStage &s, const void *src, ptrdiff_t stride, int w, int h, int bpp) {
   const size_t pitch = b200_align_up((size_t)w * bpp, 16);
-  const size_t plane_bytes = b200_align_up(pitch * h, 256);
-  B200_CUDA(ctx, cudaSetDevice(ctx->device));
-  B200_CUDA(ctx, cudaMallocAsync(&hp->dbase, 2 * plane_bytes + extra + 256, ctx->stream));
-  uint8_t *p = (uint8_t *)hp->dbase;
-  B200_CUDA(ctx, cudaMemcpy2DAsync(p, pitch, src, (size_t)ss, (size_t)w * bpp, h, cudaMemcpyHostToDevice, ctx->stream));
-  B200_CUDA(ctx, cudaMemcpy2DAsync(p + plane_bytes, pitch, dst, (size_t)ds, (size_t)w * bpp, h,
-                                   cudaMemcpyHostToDevice, ctx->stream));
-  hp->a.data = p;
-  hp->b.data = p + plane_bytes;
-  hp->a.stride = hp->b.stride = (int32_t)(pitch / bpp);
-  hp->a.width = hp->b.width = w;
-  hp->a.height = hp->b.height = h;
-  hp->a.bpp = hp->b.bpp = bpp;
-  *extra_ptr = p + 2 * plane_bytes;
-  return B200_OK;
+  b200_plane p{};
+  p.data = s.take(pitch * h);
+  p.stride = (int32_t)(pitch / bpp);
+  p.width = w;
+  p.height = h;
+  p.bpp = bpp;
+  s.up2d(p.data, pitch, src, (size_t)stride, (size_t)w * bpp, h);
+  return p;
 }
 
 }  // namespace
@@ -171,51 +161,40 @@ extern "C" uint64_t b200_weighted_sse(const void *src, ptrdiff_t src_stride, con
                                       ptrdiff_t dst_stride, const uint32_t *scale,
                                       ptrdiff_t scale_stride_bytes, int w, int h, int bpp) {
   b200_ctx *ctx = b200_default_ctx();
-  auto die = [&](const char *what) {
-    fprintf(stderr, "b200rdo: FATAL: per-call weighted_sse failed (%s): %s\n", what, b200_last_error(ctx));
-    abort();  // the reference has no error return here either; never silently wrong
-  };
   const int cw = w / 4, ch = h / 4;
-  HostPair hp;
-  uint8_t *extra = nullptr;
+  const size_t plane_bytes = b200_align_up(staged_block_bytes(w, h, bpp), 256);
   const size_t scale_bytes = b200_align_up((size_t)cw * ch * 4, 256);
-  if (stage_pair(ctx, src, src_stride, dst, dst_stride, w, h, bpp, scale_bytes + 256 + 64, &hp, &extra)) die("staging");
-  uint32_t *d_scale = (uint32_t *)extra;
-  b200_block *d_blk = (b200_block *)(extra + scale_bytes);
-  uint64_t *d_out = (uint64_t *)(extra + scale_bytes + 256);
+  HostStage s(ctx, 2 * plane_bytes + scale_bytes + 256 + 64 + 256);
+  const b200_plane a = stage_block(s, src, src_stride, w, h, bpp);
+  const b200_plane b = stage_block(s, dst, dst_stride, w, h, bpp);
+  uint32_t *d_scale = (uint32_t *)s.take((size_t)cw * ch * 4);
+  b200_block *d_blk = (b200_block *)s.take(sizeof(b200_block));
+  uint64_t *d_out = (uint64_t *)s.take(8);
   const b200_block blk{0, 0};
   uint64_t out = 0;
-  if (cudaMemcpy2DAsync(d_scale, (size_t)cw * 4, scale, (size_t)scale_stride_bytes, (size_t)cw * 4, ch,
-                        cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess ||
-      cudaMemcpyAsync(d_blk, &blk, sizeof blk, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess)
-    die("H2D");
-  if (b200_weighted_sse_dev(ctx, &hp.a, &hp.b, d_blk, 1, w, h, d_scale, (size_t)cw, d_out)) die("launch");
-  if (cudaMemcpyAsync(&out, d_out, 8, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess) die("D2H");
-  cudaFreeAsync(hp.dbase, ctx->stream);
-  if (cudaStreamSynchronize(ctx->stream) != cudaSuccess) die("sync");
+  s.up2d(d_scale, (size_t)cw * 4, scale, (size_t)scale_stride_bytes, (size_t)cw * 4, ch);
+  s.up(d_blk, &blk, sizeof blk);
+  if (s.ok()) s.run(b200_weighted_sse_dev(ctx, &a, &b, d_blk, 1, w, h, d_scale, (size_t)cw, d_out));
+  s.down(&out, d_out, 8);
+  b200_percall_check(ctx, s.finish(true), "weighted_sse");
   return out;
 }
 
 extern "C" uint32_t b200_cdef_dist_kernel(const void *src, ptrdiff_t src_stride, const void *dst,
                                           ptrdiff_t dst_stride, int w, int h, int bit_depth, uint32_t ret[3]) {
   b200_ctx *ctx = b200_default_ctx();
-  auto die = [&](const char *what) {
-    fprintf(stderr, "b200rdo: FATAL: per-call cdef_dist_kernel failed (%s): %s\n", what, b200_last_error(ctx));
-    abort();
-  };
   const int bpp = bit_depth == 8 ? 1 : 2;
-  HostPair hp;
-  uint8_t *extra = nullptr;
-  if (stage_pair(ctx, src, src_stride, dst, dst_stride, w, h, bpp, 512, &hp, &extra)) die("staging");
-  b200_block *d_blk = (b200_block *)extra;
-  uint32_t *d_out = (uint32_t *)(extra + 256);
+  HostStage s(ctx, 2 * b200_align_up(staged_block_bytes(w, h, bpp), 256) + 512 + 256);
+  const b200_plane a = stage_block(s, src, src_stride, w, h, bpp);
+  const b200_plane b = stage_block(s, dst, dst_stride, w, h, bpp);
+  b200_block *d_blk = (b200_block *)s.take(sizeof(b200_block));
+  uint32_t *d_out = (uint32_t *)s.take(16);
   const b200_block blk{0, 0};
   uint32_t host[4] = {0, 0, 0, 0};
-  if (cudaMemcpyAsync(d_blk, &blk, sizeof blk, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess) die("H2D");
-  if (b200_cdef_dist_dev(ctx, &hp.a, &hp.b, d_blk, 1, w, h, bit_depth, d_out, d_out + 1)) die("launch");
-  if (cudaMemcpyAsync(host, d_out, 16, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess) die("D2H");
-  cudaFreeAsync(hp.dbase, ctx->stream);
-  if (cudaStreamSynchronize(ctx->stream) != cudaSuccess) die("sync");
+  s.up(d_blk, &blk, sizeof blk);
+  if (s.ok()) s.run(b200_cdef_dist_dev(ctx, &a, &b, d_blk, 1, w, h, bit_depth, d_out, d_out + 1));
+  s.down(host, d_out, 16);
+  b200_percall_check(ctx, s.finish(true), "cdef_dist_kernel");
   if (ret) ret[0] = host[1], ret[1] = host[2], ret[2] = host[3];
   return host[0];
 }

@@ -15,7 +15,7 @@
 // cross-checks; the batched `_dev` entry points are the product path.
 #include <cuda_runtime.h>
 
-#include "common.cuh"
+#include "host_stage.cuh"
 
 namespace {
 
@@ -53,30 +53,19 @@ void cfl_ac(int16_t *ac, const void *src, ptrdiff_t stride, int bpp, int w_pad, 
   b200_ctx *ctx = b200_default_ctx();
   const int lw = w << xdec, lh = h << ydec;
   const size_t luma_bytes = b200_align_up((size_t)lw * lh * bpp, 256);
-  void *dbase = nullptr;
-  int st = B200_OK;
-  if (cudaSetDevice(ctx->device) != cudaSuccess ||
-      cudaMallocAsync(&dbase, luma_bytes + 256 + (size_t)w * h * 2, ctx->stream) != cudaSuccess)
-    st = b200_fail(ctx, B200_ERR_CUDA, "alloc failed");
-  b200_block *d_blk = (b200_block *)((uint8_t *)dbase + luma_bytes);
-  int16_t *d_ac = (int16_t *)((uint8_t *)dbase + luma_bytes + 256);
+  HostStage s(ctx, luma_bytes + 256 + (size_t)w * h * 2);
+  uint8_t *d_luma = s.take((size_t)lw * lh * bpp);
+  b200_block *d_blk = (b200_block *)s.take(sizeof(b200_block));
+  int16_t *d_ac = (int16_t *)s.take((size_t)w * h * 2);
   const b200_block blk{0, 0};
-  if (!st && (cudaMemcpy2DAsync(dbase, (size_t)lw * bpp, src, (size_t)stride, (size_t)lw * bpp, lh,
-                                cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess ||
-              cudaMemcpyAsync(d_blk, &blk, sizeof blk, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess))
-    st = b200_fail(ctx, B200_ERR_CUDA, "H2D copy failed");
-  if (!st) {
-    const b200_plane p{dbase, lw, lw, lh, 0, bpp, nullptr};
-    st = b200_pred_cfl_ac_dev(ctx, &p, d_blk, 1, w, h, w_pad, h_pad, xdec, ydec, d_ac);
+  s.up2d(d_luma, (size_t)lw * bpp, src, (size_t)stride, (size_t)lw * bpp, lh);
+  s.up(d_blk, &blk, sizeof blk);
+  if (s.ok()) {
+    const b200_plane p{d_luma, lw, lw, lh, 0, bpp, nullptr};
+    s.run(b200_pred_cfl_ac_dev(ctx, &p, d_blk, 1, w, h, w_pad, h_pad, xdec, ydec, d_ac));
   }
-  if (!st && cudaMemcpyAsync(ac, d_ac, (size_t)w * h * 2, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess)
-    st = b200_fail(ctx, B200_ERR_CUDA, "D2H copy failed");
-  if (dbase) cudaFreeAsync(dbase, ctx->stream);
-  if (!st && cudaStreamSynchronize(ctx->stream) != cudaSuccess) st = b200_fail(ctx, B200_ERR_CUDA, "sync failed");
-  if (st) {
-    fprintf(stderr, "b200rdo: FATAL: cfl_ac failed: %s\n", b200_last_error(ctx));
-    abort();
-  }
+  s.down(ac, d_ac, (size_t)w * h * 2);
+  b200_percall_check(ctx, s.finish(true), "cfl_ac");
 }
 
 }  // namespace

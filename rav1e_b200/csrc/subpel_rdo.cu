@@ -22,7 +22,6 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
-#include <mutex>
 
 #include "fwd_txfm_dev.cuh"
 #include "mc_dev.cuh"
@@ -218,12 +217,7 @@ int launch_srdo(b200_ctx *ctx, SrdoArgs a) {
   const size_t per_warp = b200_align_up(pred_off + 2 * (size_t)W * H * sizeof(T), 16);
   const int wpc = (int)std::min<size_t>(8, std::max<size_t>(1, (160 * 1024) / per_warp));
   const size_t smem = per_warp * wpc;
-  static std::once_flag once;
-  static cudaError_t err = cudaSuccess;
-  std::call_once(once, [] {
-    err = cudaFuncSetAttribute(subpel_rdo_kernel<T, W, H>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-  });
-  B200_CUDA(ctx, err);
+  if (int st = b200_smem_opt_in(ctx, (const void *)subpel_rdo_kernel<T, W, H>, 200 * 1024)) return st;
   a.smem_per_warp = (int)per_warp;
   a.pred_off = (int)pred_off;
   const int grid = (int)std::min<size_t>((a.nblocks + wpc - 1) / wpc, (size_t)ctx->num_sms * 16);
