@@ -637,6 +637,62 @@ def cdef_rdo(ctx):
             ctx.plane_free(p)
 
 
+def deblock(ctx):
+    """b200_deblock_levels_dev and b200_deblock_filter_dev on a 1080p 4:2:0 frame at 8 and 10 bit (seeded
+    partition, half the blocks skip), once as one frame item and once as 2x2-superblock area items, each call
+    timed on its own.  Algorithmic bytes: the level search reads rec + src over the items and the 4x4 block
+    grid; the filter reads in + the grid and writes out.  Next to it, the oracle with every host thread on the
+    same inputs (one thread per item), and a full check of levels, tallies and output against it."""
+    from tests.test_deblock_gpu import DevPlanes, frame_setup
+    from tests.test_oracle_deblock import orc_levels
+    from tests.test_oracle_deblock_spec import PAD, orc_filter, state_array
+    W, H = 1920, 1080
+    w4, h4 = W // 4, ((H + 7) >> 3) * 2
+    frame = [(0, 0, w4, h4, W, H)]
+    areas = [(x, y, min(32, w4 - x), min(32, h4 - y), W - 4 * x, H - 4 * y) for y in range(0, h4, 32)
+             for x in range(0, w4, 32)]
+    st = state_array()
+    for bd in (8, 10):
+        rng = np.random.default_rng(60 + bd)
+        grid, src, rec = frame_setup(rng, "420", bd, W, H, skip_p=0.5)
+        bpp = 1 if bd == 8 else 2
+        pix = (W * H * 3 // 2) * bpp
+        d_rec, d_src = DevPlanes(ctx, rec, "420"), DevPlanes(ctx, src, "420")
+        d_out = DevPlanes(ctx, [np.zeros_like(a) for a in rec], "420")
+        d_mi = dev(grid)
+        for label, items in (("frame item", frame), ("2x2-superblock areas", areas)):
+            n = len(items)
+            d_lv = torch.empty(n * 4, dtype=torch.uint8, device="cuda")
+            d_t = torch.empty(n * 3 * 2 * 64 * 8, dtype=torch.uint8, device="cuda")
+            lv_ms = timed(lambda: ctx.deblock_levels_dev(d_rec.views, d_src.views, 1, 1, bd, d_mi, w4, items, d_lv,
+                                                          d_t))
+            f_ms = timed(lambda: ctx.deblock_filter_dev(d_rec.views, d_out.views, 1, 1, bd, st, d_lv, d_mi, w4, items))
+            want_lv, want_t = orc_levels(rec, src, "420", bd, grid, items)
+            got_lv = d_lv.cpu().numpy().reshape(n, 4)
+            got_t = d_t.cpu().numpy().view(np.int64).reshape(n, 3, 2, 64)
+            filt = [a.copy() for a in rec]
+            orc_filter(filt, "420", bd, st, want_lv, grid, items)
+            got = d_out.download()
+
+            def visible(a, p):
+                o, w, h = PAD >> (p > 0), W >> (p > 0), H >> (p > 0)
+                return a[o:o + h, o:o + w]
+            same = bool((got_lv == want_lv).all() and (got_t == want_t).all() and
+                        all((visible(g, p) == visible(f, p)).all() for p, (g, f) in enumerate(zip(got, filt))))
+            assert same, f"deblock {label} {bd}-bit disagrees with the oracle"
+            cpu_lv = cpu_rate(lambda: orc_levels(rec, src, "420", bd, grid, items), 1)
+            cpu_f = cpu_rate(lambda: orc_filter([a.copy() for a in rec], "420", bd, st, want_lv, grid, items), 1)
+            extra = {"items": n, "bit_depth": bd, "same_as_oracle": same, "levels_mean": float(want_lv.mean()),
+                     "library": os.path.basename(B.LIB_PATH)}
+            emit(f"deblock_levels_dev {label} {bd}-bit 4:2:0 (sse_optimize)", 1, "frames", lv_ms,
+                 2 * pix + grid.nbytes, "1080p, seeded partition, half skip; bytes: rec + src + 4x4 grid",
+                 cpu=cpu_lv, extra=extra)
+            emit(f"deblock_filter_dev {label} {bd}-bit 4:2:0 (deblock_filter_frame)", 1, "frames", f_ms,
+                 2 * pix + grid.nbytes, "same frame and levels; bytes: in + out + 4x4 grid", cpu=cpu_f, extra=extra)
+        for dp in (d_rec, d_src, d_out):
+            dp.free()
+
+
 def main():
     torch.cuda.set_device(0)
     stream = torch.cuda.Stream()
@@ -657,6 +713,9 @@ def main():
         return
     if "--cfl-alpha" in sys.argv[1:]:
         cfl_alpha(ctx)
+        return
+    if "--deblock" in sys.argv[1:]:
+        deblock(ctx)
         return
     rng = np.random.default_rng(0)
     W, H, PAD = 1920, 1080, 96

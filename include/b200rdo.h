@@ -748,6 +748,74 @@ int b200_cdef_rdo_dev(b200_ctx *ctx, const b200_plane *rec, const b200_plane *sr
                       const b200_cdef_rdo_area *areas, size_t n_areas, const uint32_t *d_rate, uint64_t *d_err,
                       double *d_cost, int8_t *d_best);
 
+/* ------------------------------------------------------- deblocking (deblock.rs)
+ * The deblocking filter's level search (deblock_filter_optimize without fast_deblock, i.e. sse_optimize,
+ * deblock.rs:1461-1618) and the filter itself (deblock_filter_frame -> deblock_plane, deblock.rs:1294-1551)
+ * for a HOST list of items, each asynchronous on the context's stream.  An item is the TileBlocks rect one
+ * of the reference's call sites passes: the whole frame (encoder.rs:3263-3290), a tile (the delayed
+ * loop-filter RDO, encoder.rs:3586-3625) or a loop-restoration area (rdo.rs:2297-2331).  Edges are found on
+ * the item's own grid: nothing is filtered across its left or top border.  Levels stay on the device
+ * between the two calls, so "levels, filter, b200_cdef_rdo_dev" needs no host synchronisation.
+ *
+ * d_mi: one b200_deblock_mi per 4x4 luma block of the frame, mi_stride records per row, covering every
+ * item's mi rect.  It is device data, so it is not checked: every table lookup is bounded for any byte
+ * value, and for a record the reference would panic on (bsize >= 22, txsize >= 19, a bsize without a
+ * subsampled_size in 4:2:2) the item's results are unspecified.  The grid must be consistent as an
+ * encoder writes it (one bsize and txsize per block, transforms tiling the block): the filter runs all
+ * edges of one direction in parallel, which equals the reference's order only when no two edges of one
+ * direction touch the same pixels.
+ *
+ * The working rect of an item is the region the reference's scratch copy covers: luma pixels
+ * [4 mi_x, 4 mi_x + min(4 mi_w, vis_w rounded up to 8)) and likewise vertically; chroma planes take it
+ * decimated.  The filter reads `in` and writes `out` there and nowhere else: pixels are filtered where an
+ * edge is filtered and copied from `in` everywhere else, so a caller needs no "deblock in place, then
+ * restore" (encoder.rs:3598-3647).  An item whose luma levels are both 0 gets a copy of `in` in every plane,
+ * as every call site skips deblock_filter_frame then (encoder.rs:3280, :3598, rdo.rs:2311); a chroma plane
+ * whose own level is 0 gets a copy (deblock.rs:1302-1319).  The level search reads rec and src over the
+ * working rect and, because sse_h_edge sizes horizontal edges by the transform WIDTH (deblock.rs:1257, kept
+ * as is), up to 4 rows above and below it.
+ *
+ * rec / src / in / out: HOST arrays of `planes` (1 = 4:0:0, or 3) device planes.  d_levels: 4 per item
+ * (Y vertical, Y horizontal, U, V); the level search writes them (0 for U and V in 4:0:0), the filter reads
+ * them.  d_tally (may be NULL): per item x plane (3, zeros for absent planes) x {vertical, horizontal}, the
+ * 64 prefix-summed i64 tallies (levels 0..63) the argmin reads: d_tally[((item * 3 + p) * 2 + dir) * 64 + l].
+ * Rejected with B200_ERR_ARG before any launch, with nothing written: NULL pointers, a bpp that does not
+ * match bit_depth (8 / 10 / 12), planes other than 1 / 3, a layout other than 4:2:0 / 4:2:2 / 4:4:4, an
+ * item whose origin is not on the 64x64 superblock grid, that is empty, has an odd mi_w / mi_h (FrameBlocks
+ * are always an even number of 4x4 blocks, encoder.rs:852-853), reaches past mi_stride, or overlaps
+ * another item, vis_w / vis_h <= 0, a working rect (for the level search extended by 4 rows above and
+ * below) outside a plane's readable area [-pad, width + pad) x [-pad, height + pad), with the filter `out`
+ * aliasing `in`, and a state with block_delta_shift above 3 (delta_lf_res is two bits).
+ * n_items == 0 launches nothing. */
+typedef struct {   /* one per 4x4 luma block: the fields of Block (context/block_unit.rs:165-183) deblocking reads */
+  uint8_t bsize;   /* BlockSize 0..21 (n4_w / n4_h and the chroma tx size derive from it) */
+  uint8_t txsize;  /* luma TxSize 0..18 */
+  uint8_t mode;    /* PredictionMode discriminant (mode_deltas' mode type, deblock.rs:48-53) */
+  uint8_t skip;    /* 0 / 1 */
+  int8_t ref0;     /* ref_frames[0].to_index(); 0 = INTRA_FRAME */
+  int8_t deltas[4]; /* Block::deblock_deltas */
+  uint8_t pad_[3];
+} b200_deblock_mi; /* 12 B */
+typedef struct {
+  int32_t mi_x, mi_y; /* origin in 4x4 luma units, frame-absolute, multiples of 16 (a superblock) */
+  int32_t mi_w, mi_h; /* the item's TileBlocks cols() / rows() */
+  int32_t vis_w, vis_h; /* visible luma pixels from the origin: crop_w - rect.x, crop_h - rect.y */
+} b200_deblock_item;
+typedef struct {       /* DeblockState (encoder.rs:522-532) without levels; sharpness is not read */
+  uint8_t deltas_enabled;
+  int8_t ref_deltas[8];
+  int8_t mode_deltas[2];
+  uint8_t block_deltas_enabled, block_delta_shift, block_delta_multi;
+  uint8_t pad_[2];
+} b200_deblock_state; /* 16 B */
+int b200_deblock_levels_dev(b200_ctx *ctx, const b200_plane *rec, const b200_plane *src, int planes, int xdec,
+                            int ydec, int bit_depth, const b200_deblock_mi *d_mi, int mi_stride,
+                            const b200_deblock_item *items, size_t n_items, uint8_t *d_levels, int64_t *d_tally);
+int b200_deblock_filter_dev(b200_ctx *ctx, const b200_plane *in, const b200_plane *out, int planes, int xdec,
+                            int ydec, int bit_depth, const b200_deblock_state *state, const uint8_t *d_levels,
+                            const b200_deblock_mi *d_mi, int mi_stride, const b200_deblock_item *items,
+                            size_t n_items);
+
 /* ------------------------------------------------------- intra prediction (predict.rs)
  * Boundary = rust::dispatch_predict_intra(mode, variant, dst, tx_size, bit_depth, ac, angle,
  * ief_params, edge_buf, cpu) (predict.rs:705-784; the asm wrappers, asm/x86/predict.rs:239-873,

@@ -99,6 +99,15 @@ CFL_ITEM_DTYPE = np.dtype([("x", "<i2"), ("y", "<i2"), ("bsize", "u1"), ("tx_siz
 assert CFL_ITEM_DTYPE.itemsize == 8
 CFL_ALPHAS = 33              # b200_cfl_alpha_dev's d_sse entries per (item, chroma plane): alpha -16 ..= 16
 INTER_SCREEN_SINGLE = 0xFF   # b200_inter_screen_cand.ref[1] of a single-reference entry (NONE_FRAME)
+# b200_deblock_mi / b200_deblock_item / b200_deblock_state (include/b200rdo.h)
+DEBLOCK_MI_DTYPE = np.dtype([("bsize", "u1"), ("txsize", "u1"), ("mode", "u1"), ("skip", "u1"), ("ref0", "i1"),
+                             ("deltas", "i1", (4,)), ("pad_", "u1", (3,))])
+DEBLOCK_ITEM_DTYPE = np.dtype([("mi_x", "<i4"), ("mi_y", "<i4"), ("mi_w", "<i4"), ("mi_h", "<i4"), ("vis_w", "<i4"),
+                               ("vis_h", "<i4")])
+DEBLOCK_STATE_DTYPE = np.dtype([("deltas_enabled", "u1"), ("ref_deltas", "i1", (8,)), ("mode_deltas", "i1", (2,)),
+                                ("block_deltas_enabled", "u1"), ("block_delta_shift", "u1"),
+                                ("block_delta_multi", "u1"), ("pad_", "u1", (2,))])
+assert DEBLOCK_MI_DTYPE.itemsize == 12 and DEBLOCK_ITEM_DTYPE.itemsize == 24 and DEBLOCK_STATE_DTYPE.itemsize == 16
 ME_RESULT_DTYPE = np.dtype(
     {"names": ["cost", "sad", "mv_row", "mv_col"],
      "formats": ["<u8", "<u4", "<i2", "<i2"], "offsets": [0, 8, 12, 14], "itemsize": 16})
@@ -251,6 +260,8 @@ def lib():
     L.b200_inter_mode_screen_dev.argtypes = [vp, pp] + [i32] * 4 + [vp] + [i32] * 5 + [vp, sz, vp, vp]
     L.b200_cdef_rdo_dev.argtypes = [vp, vp, vp, vp] + [i32] * 8 + [vp] * 5 + [C.c_double, vp, sz, vp, vp, vp, vp]
     L.b200_cfl_alpha_dev.argtypes = [vp, vp, vp] + [i32] * 9 + [vp, sz, vp, vp]
+    L.b200_deblock_levels_dev.argtypes = [vp, vp, vp] + [i32] * 4 + [vp, i32, vp, sz, vp, vp]
+    L.b200_deblock_filter_dev.argtypes = [vp, vp, vp] + [i32] * 4 + [vp, vp, vp, i32, vp, sz]
     _LIB = L
     return L
 
@@ -531,6 +542,42 @@ class Context:
             width, height, bit_depth, damping, cdef_bits, C.addressof(ys), C.addressof(us), _dev_ptr(d_skip8),
             _dev_ptr(d_imp_scales), C.addressof(ds), float(lam), ar.ctypes.data, len(areas), _dev_ptr(d_rate),
             _dev_ptr(d_err), _dev_ptr(d_cost), _dev_ptr(d_best)))
+
+    # ---- deblocking
+    @staticmethod
+    def _plane_array(planes):
+        a = (Plane * len(planes))()
+        for k, p in enumerate(planes):
+            C.memmove(C.byref(a[k]), C.byref(p), C.sizeof(Plane))
+        return a
+
+    @staticmethod
+    def _deblock_items(items):
+        """DEBLOCK_ITEM_DTYPE records or rows of six ints -> a contiguous (n, 6) int32 array."""
+        a = np.ascontiguousarray(items)
+        if a.dtype.names:
+            a = a.view(np.int32)
+        return np.ascontiguousarray(np.asarray(a, np.int32).reshape(-1, 6))
+
+    def deblock_levels_dev(self, rec, src, xdec, ydec, bit_depth, d_mi, mi_stride, items, d_levels, d_tally=None):
+        """rec / src: lists of 1 or 3 Plane; d_mi: DEBLOCK_MI_DTYPE records on the device, mi_stride per row;
+        items: a host DEBLOCK_ITEM_DTYPE array (or rows of (mi_x, mi_y, mi_w, mi_h, vis_w, vis_h)); d_levels
+        (4 u8 per item) and d_tally (items x 3 x 2 x 64 i64, may be None) on the device (include/b200rdo.h)."""
+        r, s_ = self._plane_array(rec), self._plane_array(src)
+        it = self._deblock_items(items)
+        self.check(self.L.b200_deblock_levels_dev(self.h, C.addressof(r), C.addressof(s_), len(rec), xdec, ydec,
+                                                  bit_depth, _dev_ptr(d_mi), mi_stride, it.ctypes.data, len(it),
+                                                  _dev_ptr(d_levels), _dev_ptr(d_tally)))
+
+    def deblock_filter_dev(self, inp, out, xdec, ydec, bit_depth, state, d_levels, d_mi, mi_stride, items):
+        """inp / out: lists of 1 or 3 Plane; state: a DEBLOCK_STATE_DTYPE scalar array; d_levels: 4 u8 per item
+        on the device; the rest as deblock_levels_dev."""
+        i_, o = self._plane_array(inp), self._plane_array(out)
+        it = self._deblock_items(items)
+        st = np.ascontiguousarray(np.asarray(state, DEBLOCK_STATE_DTYPE).reshape(1))
+        self.check(self.L.b200_deblock_filter_dev(self.h, C.addressof(i_), C.addressof(o), len(inp), xdec, ydec,
+                                                  bit_depth, st.ctypes.data, _dev_ptr(d_levels), _dev_ptr(d_mi),
+                                                  mi_stride, it.ctypes.data, len(it)))
 
     # ---- intra prediction
     def predict_intra_dev(self, d_edges, d_items, n, d_ac, w, h, bit_depth, plane_w, plane_h, d_out):
