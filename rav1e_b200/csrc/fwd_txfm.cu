@@ -129,6 +129,266 @@ __global__ void __launch_bounds__(kTxThreads) fwd_txfm_kernel(const __grid_const
   }
 }
 
+// ---------------------------------------------------------------- DCT_DCT from aligned planes
+// The fused-residual forms on 8-bit planes at DCT_DCT with both sides in 8..32 take a kernel of their
+// own: the 1-D kinds, the absence of flips and the three stage shifts (forward_shared.rs:22-64,
+// classes A and B of kShiftClass) are compile-time, and each block row is read as whole 16-byte
+// segments, one round of blocks ahead of the one being transformed.  A warp owns its blocks end to
+// end, so it needs no __syncthreads:
+//   rows:    lane t loads row t of cur and of the prediction (aligned 16-byte segments, the bytes
+//            picked out with funnel shifts), forms the residual, stores it as a row of the tile;
+//   columns: lane c runs the column transform on column c (forward.rs:95-126) in place;
+//   rows:    lane t runs the row transform on row t (forward.rs:131-160) and stages its outputs in
+//            the block's coefficient order dst[k * H + t] (forward.rs:135-159 for W, H <= 32);
+//   store:   the lanes write the block's contiguous W * H coefficients with 16-byte stores.
+// The block records, winner vectors and pair lookups of up to 32 blocks are resolved once, one
+// block per lane, and handed to the lanes that transform the block by shuffles.
+//
+// forward_shared.rs:22-64 at 8 bit: av1_round_shift_array `bit` = -shift[k] (TxSetup::bit0..2)
+template <int W, int H>
+struct FastShift {
+  static constexpr bool kClassB = W * H >= 512;  // 32x32, 16x32, 32x16
+  static constexpr int bit0 = -4, bit1 = kClassB ? 2 : 1, bit2 = 0;
+};
+
+template <int BIT>
+__device__ __forceinline__ int round_shift_c(int v) {
+  if constexpr (BIT > 0) return (v + (1 << (BIT - 1))) >> BIT;
+  else return (int)((unsigned)v << (-BIT));
+}
+
+template <int N>
+__device__ __forceinline__ void fdct_1d(TXV (&c)[N]) {
+  if constexpr (N == 8) tx_fdct8(c);
+  else if constexpr (N == 16) tx_fdct16(c);
+  else tx_fdct32(c);
+}
+
+// RB bytes from p (any alignment), read only through the 16-byte-aligned segments that hold them:
+// such a segment lies inside the 16-byte granules of the row, so it stays in the allocation whenever
+// the row's start and pitch are 16-byte aligned.  fetch() issues the loads, bytes() picks the row out
+// of the segments once they have arrived, so a round's loads can be in flight during the previous one.
+template <int RB>
+struct RowSegs {
+  static constexpr int NW = RB / 4, NSEG = RB >= 16 ? RB / 16 + 1 : 2;
+  uint32_t w[NSEG * 4];
+  int off;
+
+  __device__ __forceinline__ void fetch(const uint8_t *p) {
+    off = (int)((uintptr_t)p & 15);
+    const uint4 *s = (const uint4 *)(p - off);
+#pragma unroll
+    for (int k = 0; k < NSEG; k++) {
+      // the last segment is needed only when the row crosses into it
+      const bool need = k < NSEG - 1 || off + RB > 16 * k;
+      const uint4 v = need ? __ldg(s + k) : make_uint4(0, 0, 0, 0);
+      w[4 * k] = v.x, w[4 * k + 1] = v.y, w[4 * k + 2] = v.z, w[4 * k + 3] = v.w;
+    }
+  }
+
+  __device__ __forceinline__ void bytes(uint32_t (&o)[NW]) const {
+    uint32_t v[NSEG * 4];
+#pragma unroll
+    for (int i = 0; i < NSEG * 4; i++) v[i] = w[i];
+    if (off == 0) {
+#pragma unroll
+      for (int i = 0; i < NW; i++) o[i] = v[i];
+      return;
+    }
+    // v[i] = w[i + q] for i <= NW (two select stages), then o[i] = bytes (off & 3) .. of v[i], v[i + 1]
+    const int q = off >> 2;
+#pragma unroll
+    for (int i = 0; i < NW + 2; i++) v[i] = (q & 2) ? v[i + 2] : v[i];
+#pragma unroll
+    for (int i = 0; i < NW + 1; i++) v[i] = (q & 1) ? v[i + 1] : v[i];
+#pragma unroll
+    for (int i = 0; i < NW; i++) o[i] = __funnelshift_r(v[i], v[i + 1], (off & 3) * 8);
+  }
+};
+
+__device__ __forceinline__ int byte_at(const uint32_t *w, int c) {
+  return (int)__byte_perm(w[c >> 2], 0, 0x4440 | (c & 3));
+}
+
+constexpr int kFastThreads = 128;
+// blocks with sides up to 16 fit 80 registers with the next round's rows in flight: 6 CTAs per SM
+template <int W, int H>
+constexpr int fast_min_ctas() { return W <= 16 && H <= 16 ? 6 : 1; }
+
+template <int W, int H>
+__global__ void __launch_bounds__(kFastThreads, fast_min_ctas<W, H>()) fwd_dct_fast_kernel(const __grid_constant__ TxArgs a) {
+  using CoefT = int16_t;
+  using S = FastShift<W, H>;
+  constexpr int T = W > H ? W : H;  // lanes per block
+  constexpr int SPW = 32 / T;       // blocks per warp round
+  constexpr int PITCH = W + 4;      // keeps rows 16-byte aligned; row and column accesses conflict-free
+  // slot s starts at bank 8s (8x8), 16s (16-wide) so the slots of a warp use disjoint banks
+  constexpr int SLOT = (H * PITCH + 31) / 32 * 32 + (SPW > 1 ? T : 0);
+  constexpr int WARPS = kFastThreads / 32;
+  constexpr int RB = W;  // bytes per block row
+  static_assert(W * H * sizeof(CoefT) <= H * PITCH * 4, "coefficients fit the tile");
+  __shared__ __align__(16) int smem[WARPS][SPW * SLOT];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int slot = lane / T, t = lane - slot * T;
+  int *tile = smem[warp] + slot * SLOT;
+  const size_t coef_bytes = (size_t)W * H * sizeof(CoefT);
+  // Round r of the launch is blocks [r * SPW, r * SPW + SPW); warp w of tw takes rounds w, w + tw, ...,
+  // so the warps on the GPU at one time work on neighbouring blocks (and the same reference area).
+  // A pass of a warp is its next RPP rounds, whose blocks are resolved one per lane up front.
+  constexpr int RPP = 32 / SPW;
+  // (32-bit indices: the host sends fewer than 2^31 blocks)
+  const uint32_t n = (uint32_t)a.n, rounds = (n + SPW - 1) / SPW;
+  const uint32_t tw = gridDim.x * WARPS, w = blockIdx.x * WARPS + warp;
+  const uint32_t my_rounds = w < rounds ? (rounds - w + tw - 1) / tw : 0;
+  const auto block_of = [&](uint32_t p0, int j) { return ((p0 + j / SPW) * tw + w) * SPW + j % SPW; };
+  for (uint32_t p0 = 0; p0 < my_rounds; p0 += RPP) {
+    const int nloc = (int)min((uint32_t)RPP, my_rounds - p0) * SPW;
+    // lane j: where the rows of block block_of(p0, j) start (NULL: no such block)
+    const uint8_t *cur_p = nullptr, *ref_p = nullptr;
+    int cur_sb = 0, ref_sb = 0;  // row pitches, bytes
+    if (lane < nloc && block_of(p0, lane) < n) {
+      const uint32_t blk = block_of(p0, lane);
+      const b200_block b = a.blocks[blk];
+      int dx = 0, dy = 0;
+      if (a.mv_src) {
+        const b200_me_result m = a.mv_src[blk];
+        if (m.cost != ~0ull) dx = m.mv_col / 8, dy = m.mv_row / 8;
+      }
+      const void *cp = a.cur, *rp = a.ref;
+      int cs = a.cur_stride, rs = a.ref_stride;
+      if (a.pr.n > 1) {  // first pair whose block range holds blk
+        int lo = 0, hi = a.pr.n - 1;
+        while (lo < hi) {
+          const int mid = (lo + hi) >> 1;
+          if ((uint32_t)blk < a.pr.block_end[mid])
+            hi = mid;
+          else
+            lo = mid + 1;
+        }
+        cp = a.pr.cur[lo], rp = a.pr.ref[lo];
+        cs = a.pr.cur_stride[lo], rs = a.pr.ref_stride[lo];
+      }
+      cur_p = (const uint8_t *)cp + (long long)b.y * cs + b.x;
+      cur_sb = cs;
+      if (a.pred_packed) {
+        ref_p = (const uint8_t *)a.pred_packed + (size_t)blk * (W * H);
+        ref_sb = RB;
+      } else {
+        ref_p = (const uint8_t *)rp + (long long)(b.y + dy) * rs + b.x + dx;
+        ref_sb = rs;
+      }
+    }
+    // round i + SPW's rows are loaded while round i is transformed
+    RowSegs<RB> next_cur, next_ref;
+    const auto fetch = [&](int i) {
+      const int j = i + slot;
+      const uint8_t *cp = (const uint8_t *)__shfl_sync(~0u, (unsigned long long)cur_p, j);
+      const uint8_t *rp = (const uint8_t *)__shfl_sync(~0u, (unsigned long long)ref_p, j);
+      const int cs = __shfl_sync(~0u, cur_sb, j), rs = __shfl_sync(~0u, ref_sb, j);
+      if (cp && t < H) {
+        next_cur.fetch(cp + (long long)t * cs);
+        next_ref.fetch(rp + (long long)t * rs);
+      }
+    };
+    fetch(0);
+    for (int i = 0; i < nloc; i += SPW) {
+      const uint32_t blk = block_of(p0, i + slot);
+      const bool valid = blk < n;
+      const RowSegs<RB> row_cur = next_cur, row_ref = next_ref;
+      if (i + SPW < nloc) fetch(i + SPW);
+      // ---- residual rows (encoder.rs:1533 `diff`)
+      if (valid && t < H) {
+        uint32_t cw[RB / 4], rw[RB / 4];
+        row_cur.bytes(cw);
+        row_ref.bytes(rw);
+        int d[W];
+#pragma unroll
+        for (int c = 0; c < W; c++) d[c] = round_shift_c<S::bit0>(byte_at(cw, c) - byte_at(rw, c));
+#pragma unroll
+        for (int c = 0; c < W; c += 4) *(int4 *)&tile[t * PITCH + c] = make_int4(d[c], d[c + 1], d[c + 2], d[c + 3]);
+      }
+      __syncwarp();
+      // ---- columns (forward.rs:95-126)
+      if (valid && t < W) {
+        TXV v[H];
+#pragma unroll
+        for (int r = 0; r < H; r++) v[r] = tile[r * PITCH + t];
+        fdct_1d<H>(v);
+#pragma unroll
+        for (int r = 0; r < H; r++) tile[r * PITCH + t] = round_shift_c<S::bit1>(v[r]);
+      }
+      __syncwarp();
+      // ---- rows (forward.rs:131-160)
+      TXV v[W];
+      if (valid && t < H) {
+#pragma unroll
+        for (int k = 0; k < W; k += 4) {
+          const int4 q = *(const int4 *)&tile[t * PITCH + k];
+          v[k] = q.x, v[k + 1] = q.y, v[k + 2] = q.z, v[k + 3] = q.w;
+        }
+        fdct_1d<W>(v);
+      }
+      __syncwarp();
+      if (valid && t < H) {
+        CoefT *o = (CoefT *)tile;
+#pragma unroll
+        for (int k = 0; k < W; k++) o[k * H + t] = (CoefT)round_shift_c<S::bit2>(v[k]);
+      }
+      __syncwarp();
+      if (valid) {
+        constexpr int NCH = W * H * (int)sizeof(CoefT) / 16;
+        uint4 *dst = (uint4 *)((uint8_t *)a.out + (size_t)blk * coef_bytes);
+#pragma unroll
+        for (int q = t; q < NCH; q += T) dst[q] = ((const uint4 *)tile)[q];
+      }
+      __syncwarp();
+    }
+  }
+}
+
+template <int W, int H>
+int launch_fast(b200_ctx *ctx, const TxArgs &a) {
+  constexpr int T = W > H ? W : H;
+  constexpr int SPW = 32 / T;
+  constexpr int WARPS = kFastThreads / 32;
+  // As many CTAs as are resident at once (the rounds are spread over the warps, not the CTAs over
+  // time), fewer when there are not enough rounds for them.
+  static int per_sm[64];
+  int &occ = per_sm[ctx->device & 63];
+  if (!occ)
+    B200_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fwd_dct_fast_kernel<W, H>, kFastThreads, 0));
+  const size_t rounds = (a.n + SPW - 1) / SPW;
+  const int grid = (int)std::max<size_t>(1, std::min<size_t>((rounds + WARPS - 1) / WARPS, (size_t)ctx->num_sms * occ));
+  fwd_dct_fast_kernel<W, H><<<grid, kFastThreads, 0, ctx->stream>>>(a);
+  B200_LAUNCH_CHECK(ctx);
+  return B200_OK;
+}
+
+bool rows_16b_aligned(const void *p, long long pitch_bytes) {
+  return (uintptr_t)p % 16 == 0 && pitch_bytes % 16 == 0;
+}
+
+// The fast kernel serves a fused-residual call on 8-bit planes at DCT_DCT, sides in 8..32, when every
+// plane row and the output start on 16-byte boundaries; everything else runs fwd_txfm_kernel.  At 10
+// and 12 bit the u16 rows and i32 coefficients need about 100 registers with a round of rows in
+// flight, and fwd_txfm_kernel stayed faster there (16x16 on H100: 0.216 vs 0.291 ms per launch).
+bool fast_path_ok(const TxArgs &a, int tx_type, int w, int h, int bpp) {
+  if (!a.cur || bpp != 1 || tx_type != TX_DCT_DCT || w < 8 || h < 8 || w > 32 || h > 32) return false;
+  if (a.n >= (1u << 31)) return false;
+  if ((uintptr_t)a.out % 16) return false;
+  // packed predictions: each block is W * H >= 64 bytes, so an aligned buffer keeps every segment inside it
+  if (a.pred_packed) return rows_16b_aligned(a.pred_packed, 0) && rows_16b_aligned(a.cur, (long long)a.cur_stride * bpp);
+  if (a.pr.n > 1) {
+    for (int k = 0; k < a.pr.n; k++)
+      if (!rows_16b_aligned(a.pr.cur[k], (long long)a.pr.cur_stride[k] * bpp) ||
+          !rows_16b_aligned(a.pr.ref[k], (long long)a.pr.ref_stride[k] * bpp))
+        return false;
+    return true;
+  }
+  return rows_16b_aligned(a.cur, (long long)a.cur_stride * bpp) &&
+         rows_16b_aligned(a.ref, (long long)a.ref_stride * bpp);
+}
+
 template <int W, int H>
 int launch_txfm(b200_ctx *ctx, const TxArgs &a, int coeff_is_i32) {
   constexpr int T = W > H ? W : H;
@@ -199,6 +459,23 @@ static int fwd_txfm_impl(b200_ctx *ctx, const b200_plane *cur, const b200_plane 
   a.bit0 = ts.bit0;
   a.bit1 = ts.bit1;
   a.bit2 = ts.bit2;
+  if (fast_path_ok(a, tx_type, w, h, cur ? cur->bpp : 0)) {
+    switch (tx_size) {
+#define B200_TX(ID, W_, H_) \
+  case ID:                  \
+    return launch_fast<W_, H_>(ctx, a);
+      B200_TX(1, 8, 8)
+      B200_TX(2, 16, 16)
+      B200_TX(3, 32, 32)
+      B200_TX(7, 8, 16)
+      B200_TX(8, 16, 8)
+      B200_TX(9, 16, 32)
+      B200_TX(10, 32, 16)
+      B200_TX(15, 8, 32)
+      B200_TX(16, 32, 8)
+#undef B200_TX
+    }
+  }
   switch (tx_size) {
 #define B200_TX(ID, W_, H_) \
   case ID:                  \
