@@ -693,6 +693,43 @@ def deblock(ctx):
             dp.free()
 
 
+def lrf(ctx):
+    """b200_lrf_filter_dev on a 1080p 4:2:0 frame at 8 and 10 bit (seeded smooth content plus noise), with the
+    two unit configurations RestorationState::new gives 1080p (small: luma 64 / chroma 32 at low base_q_idx;
+    large: 256 / 256 at base_q_idx above 200) and three unit mixes: all Sgrproj (what rav1e emits), all Wiener,
+    and None / Wiener / Sgrproj drawn at random.  Algorithmic bytes: cdeffed read and out written over the
+    crop; the deblocked frame's reads (a few rows per stripe) are left out.  Next to it, the oracle on one host
+    thread on the same inputs, and a full check of the output against it."""
+    from tests.test_lrf_gpu import DevPlanes
+    from tests.test_oracle_lrf_spec import PAD, make_frame, orc_lrf, random_units, unit_grid
+    W, H = 1920, 1080
+    for bd in (8, 10):
+        rng = np.random.default_rng(70 + bd)
+        cd, db = make_frame(rng, W, H, "420", bd, "smooth")
+        bpp = 1 if bd == 8 else 2
+        pix = (W * H + 2 * (W // 2) * (H // 2)) * bpp
+        d_cd, d_db = DevPlanes(ctx, cd), DevPlanes(ctx, db)
+        d_out = DevPlanes(ctx, [np.zeros_like(a) for a in cd])
+        for cfg, us in (("small units 64/32", [64, 32, 32]), ("large units 256/256", [256, 256, 256])):
+            for mix, kinds in (("all sgrproj", (2,)), ("all wiener", (1,)), ("mixed", (0, 1, 2))):
+                units = [random_units(rng, *unit_grid(W, H, p, "420", us[p]), kinds=kinds) for p in range(3)]
+                ms = timed(lambda: ctx.lrf_filter_dev(d_cd.views, d_db.views, d_out.views, 1, 1, W, H, bd, 1, us,
+                                                      units))
+                want = orc_lrf(cd, db, "420", bd, W, H, 1, us, units)
+                got = d_out.download()
+                same = all((g[PAD:PAD + (H >> (p > 0)), PAD:PAD + (W >> (p > 0))] ==
+                            w[PAD:PAD + (H >> (p > 0)), PAD:PAD + (W >> (p > 0))]).all()
+                           for p, (g, w) in enumerate(zip(got, want)))
+                assert same, f"lrf {cfg} {mix} {bd}-bit disagrees with the oracle"
+                cpu = cpu_rate(lambda: orc_lrf(cd, db, "420", bd, W, H, 1, us, units), 1)
+                extra = {"bit_depth": bd, "unit_size": us, "units": mix, "same_as_oracle": same,
+                         "library": os.path.basename(B.LIB_PATH)}
+                emit(f"lrf_filter_dev {cfg} {mix} {bd}-bit 4:2:0 (lrf_filter_frame)", 1, "frames", ms, 2 * pix,
+                     "1080p seeded; bytes: cdeffed + out over the crop", cpu=cpu, extra=extra)
+        for dp in (d_cd, d_db, d_out):
+            dp.free()
+
+
 def main():
     torch.cuda.set_device(0)
     stream = torch.cuda.Stream()
@@ -716,6 +753,9 @@ def main():
         return
     if "--deblock" in sys.argv[1:]:
         deblock(ctx)
+        return
+    if "--lrf" in sys.argv[1:]:
+        lrf(ctx)
         return
     rng = np.random.default_rng(0)
     W, H, PAD = 1920, 1080, 96

@@ -816,6 +816,41 @@ int b200_deblock_filter_dev(b200_ctx *ctx, const b200_plane *in, const b200_plan
                             const b200_deblock_mi *d_mi, int mi_stride, const b200_deblock_item *items,
                             size_t n_items);
 
+/* ------------------------------------------------------- loop restoration (lrf.rs)
+ * RestorationState::lrf_filter_frame (lrf.rs:1482-1585), asynchronous on the context's stream: Wiener
+ * (wiener_stripe_filter, :1099-1207) and self-guided (setup_integral_image + sgrproj_stripe_filter,
+ * :529-830) units over whole frames, stripe by stripe, reading the CDEF output `cdeffed` and the deblocked
+ * frame `deblocked` through the reference's stripe source rules.  Planes: 1 (4:0:0) or 3; the crop of plane
+ * p is ((frame_width + (1 << xd >> 1)) >> xd) x ((frame_height + (1 << yd >> 1)) >> yd).
+ *
+ * Every pixel of every plane's crop is written to `out`, filtered or copied from `cdeffed` (None units, and
+ * Sgrproj units when enable_cdef == 0, as lrf.rs:1545-1547 skips them); nothing else is written, so a
+ * caller needs no "copy, then filter in place".  Where the frame is shorter than stripe 0 (crop_h < 56 >>
+ * ydec) the reference also writes Sgrproj rows below the crop; this call does not.  `cdeffed` may be the
+ * same plane as `deblocked`; `out` may alias neither.
+ *
+ * units[p]: a HOST array of cols x rows records for plane p, row-major, with cols = max(1, (crop_w +
+ * unit_size[p] / 2) / unit_size[p]) and rows likewise (lrf.rs:1431-1440).  A stripe's unit row is
+ * min(stripe * stripe_height / unit_size, rows - 1), with stripe_height 32 for 4:2:0 chroma and 64
+ * otherwise (lrf.rs:1295-1312); the last unit column stretches to the crop.  All records go up in one copy.
+ * Rejected with B200_ERR_ARG before any launch, with nothing written: NULL pointers, a bpp that does not
+ * match bit_depth (8 / 10 / 12), planes other than 1 / 3, a layout other than 4:2:0 / 4:2:2 / 4:4:4, a frame
+ * under 32x32 (enable_restoration_filters, encoder.rs:232), a unit_size that is not a power of two in
+ * 32..256, a plane smaller than its crop, an `out` plane's crop overlapping an input plane's crop, and a
+ * record out of range (lrf.rs:39-48): type above 2, or for Sgrproj a set above 15 or xqd outside
+ * SGRPROJ_XQD_MIN..MAX, or for Wiener a tap outside WIENER_TAPS_MIN..MAX. */
+typedef struct {      /* RestorationFilter (lrf.rs:126-136) */
+  uint8_t type;       /* 0 None, 1 Wiener, 2 Sgrproj */
+  uint8_t set;        /* Sgrproj: SGRPROJ_PARAMS_S index */
+  int8_t xqd[2];      /* Sgrproj */
+  int8_t coeffs[2][3]; /* Wiener: [0] vertical, [1] horizontal */
+  uint8_t pad_[2];
+} b200_lrf_unit;      /* 12 B */
+int b200_lrf_filter_dev(b200_ctx *ctx, const b200_plane *cdeffed, const b200_plane *deblocked,
+                        const b200_plane *out, int planes, int xdec, int ydec, int frame_width, int frame_height,
+                        int bit_depth, int enable_cdef, const int unit_size[3],
+                        const b200_lrf_unit *const units[3]);
+
 /* ------------------------------------------------------- intra prediction (predict.rs)
  * Boundary = rust::dispatch_predict_intra(mode, variant, dst, tx_size, bit_depth, ac, angle,
  * ief_params, edge_buf, cpu) (predict.rs:705-784; the asm wrappers, asm/x86/predict.rs:239-873,

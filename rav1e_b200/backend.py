@@ -108,6 +108,10 @@ DEBLOCK_STATE_DTYPE = np.dtype([("deltas_enabled", "u1"), ("ref_deltas", "i1", (
                                 ("block_deltas_enabled", "u1"), ("block_delta_shift", "u1"),
                                 ("block_delta_multi", "u1"), ("pad_", "u1", (2,))])
 assert DEBLOCK_MI_DTYPE.itemsize == 12 and DEBLOCK_ITEM_DTYPE.itemsize == 24 and DEBLOCK_STATE_DTYPE.itemsize == 16
+# b200_lrf_unit (include/b200rdo.h): type 0 None, 1 Wiener, 2 Sgrproj
+LRF_UNIT_DTYPE = np.dtype([("type", "u1"), ("set", "u1"), ("xqd", "i1", (2,)), ("coeffs", "i1", (2, 3)),
+                           ("pad_", "u1", (2,))])
+assert LRF_UNIT_DTYPE.itemsize == 12
 ME_RESULT_DTYPE = np.dtype(
     {"names": ["cost", "sad", "mv_row", "mv_col"],
      "formats": ["<u8", "<u4", "<i2", "<i2"], "offsets": [0, 8, 12, 14], "itemsize": 16})
@@ -262,6 +266,7 @@ def lib():
     L.b200_cfl_alpha_dev.argtypes = [vp, vp, vp] + [i32] * 9 + [vp, sz, vp, vp]
     L.b200_deblock_levels_dev.argtypes = [vp, vp, vp] + [i32] * 4 + [vp, i32, vp, sz, vp, vp]
     L.b200_deblock_filter_dev.argtypes = [vp, vp, vp] + [i32] * 4 + [vp, vp, vp, i32, vp, sz]
+    L.b200_lrf_filter_dev.argtypes = [vp, vp, vp, vp] + [i32] * 7 + [vp, vp]
     _LIB = L
     return L
 
@@ -578,6 +583,20 @@ class Context:
         self.check(self.L.b200_deblock_filter_dev(self.h, C.addressof(i_), C.addressof(o), len(inp), xdec, ydec,
                                                   bit_depth, st.ctypes.data, _dev_ptr(d_levels), _dev_ptr(d_mi),
                                                   mi_stride, it.ctypes.data, len(it)))
+
+    # ---- loop restoration
+    def lrf_filter_dev(self, cdeffed, deblocked, out, xdec, ydec, frame_w, frame_h, bit_depth, enable_cdef,
+                       unit_size, units):
+        """cdeffed / deblocked / out: lists of 1 or 3 Plane; unit_size: one per plane; units: one host
+        LRF_UNIT_DTYPE array per plane, (rows, cols) or flat in row-major order (include/b200rdo.h)."""
+        c_, d_, o = self._plane_array(cdeffed), self._plane_array(deblocked), self._plane_array(out)
+        n = len(cdeffed)
+        recs = [np.ascontiguousarray(np.asarray(u, LRF_UNIT_DTYPE).reshape(-1)) for u in units]
+        us = (C.c_int * 3)(*[int(v) for v in unit_size], *([0] * (3 - len(unit_size))))
+        ptrs = (C.c_void_p * 3)(*[r.ctypes.data for r in recs], *([None] * (3 - len(recs))))
+        self.check(self.L.b200_lrf_filter_dev(self.h, C.addressof(c_), C.addressof(d_), C.addressof(o), n, xdec, ydec,
+                                              frame_w, frame_h, bit_depth, int(enable_cdef), C.addressof(us),
+                                              C.addressof(ptrs)))
 
     # ---- intra prediction
     def predict_intra_dev(self, d_edges, d_items, n, d_ac, w, h, bit_depth, plane_w, plane_h, d_out):
