@@ -730,6 +730,44 @@ def lrf(ctx):
             dp.free()
 
 
+def lrf_search(ctx):
+    """b200_lrf_search_dev on a 1080p 4:2:0 frame at 8 and 10 bit (seeded smooth content plus noise), every item
+    of the frame in one call, for the three unit configurations RestorationState::new picks by base_q_idx (luma
+    64 / 128 / 256, chroma half), with the Full and the Reduced set lists.  Algorithmic bytes: lrf_in and src
+    read once per item over its unit.  Next to it, orc_lrf_search on one host thread on the same inputs, and a
+    full check of every output against it."""
+    from tests.test_oracle_lrf_search import areas_and_items, lrf_search as orc_search, make_frame
+    W, H = 1920, 1080
+    for bd in (8, 10):
+        rng = np.random.default_rng(80 + bd)
+        lin, src = make_frame(rng, W, H, "420", bd)
+        bpp = 1 if bd == 8 else 2
+        pix = (W * H + 2 * (W // 2) * (H // 2)) * bpp
+        d_in = [ctx.plane_from_host(a, 8) for a in lin]
+        d_src = [ctx.plane_from_host(a, 8) for a in src]
+        for uy in (64, 128, 256):
+            us = [uy, uy >> 1, uy >> 1]
+            areas, items = areas_and_items(rng, W, H, "420", us, incoming="mixed")
+            n = len(items)
+            d_best, d_cost, d_ch = dev(np.zeros(12 * n, np.uint8)), dev(np.zeros(n)), dev(np.zeros(n, np.uint8))
+            for reduced in (0, 1):
+                ms = timed(lambda: ctx.lrf_search_dev(d_in, d_src, 1, 1, W, H, bd, us, reduced, None, (16384,) * 3,
+                                                      500.0, areas, items, d_best, d_cost, d_ch))
+                want = orc_search(lin, src, "420", W, H, bd, us, reduced, areas, items, lam=500.0)
+                same = bool((d_best.cpu().numpy().view(np.uint8) == want[0].view(np.uint8)).all() and
+                            (d_cost.cpu().numpy().view(np.uint64) == want[1].view(np.uint64)).all() and
+                            (d_ch.cpu().numpy() == want[2]).all())
+                assert same, f"lrf_search {uy} reduced={reduced} {bd}-bit disagrees with the oracle"
+                cpu = cpu_rate(lambda: orc_search(lin, src, "420", W, H, bd, us, reduced, areas, items, lam=500.0), 1)
+                extra = {"bit_depth": bd, "unit_size": us, "sets": "reduced" if reduced else "full", "items": n,
+                         "same_as_oracle": same, "library": os.path.basename(B.LIB_PATH)}
+                emit(f"lrf_search_dev units {uy}/{uy >> 1} {'reduced' if reduced else 'full'} sets {bd}-bit 4:2:0",
+                     1, "frames", ms, 2 * pix, "1080p seeded, every item in one call; bytes: lrf_in + src once",
+                     cpu=cpu, extra=extra)
+        for p in d_in + d_src:
+            ctx.plane_free(p)
+
+
 def main():
     torch.cuda.set_device(0)
     stream = torch.cuda.Stream()
@@ -756,6 +794,9 @@ def main():
         return
     if "--lrf" in sys.argv[1:]:
         lrf(ctx)
+        return
+    if "--lrf-search" in sys.argv[1:]:
+        lrf_search(ctx)
         return
     rng = np.random.default_rng(0)
     W, H, PAD = 1920, 1080, 96

@@ -851,6 +851,70 @@ int b200_lrf_filter_dev(b200_ctx *ctx, const b200_plane *cdeffed, const b200_pla
                         int bit_depth, int enable_cdef, const int unit_size[3],
                         const b200_lrf_unit *const units[3]);
 
+/* The restoration search of one rdo_loop_decision pass (rdo.rs:2575-2740) for a HOST list of items,
+ * asynchronous on the context's stream with a fixed number of launches and no host synchronisation.  An
+ * item is one (area, plane, unit) the reference reaches at rdo.rs:2607-2611: the caller builds the list
+ * where rdo.rs:2585-2611 loops, so lru_skip / lru_on_skip and has_restoration_unit(.., false) stay with it.
+ *
+ * Per item, in the plane's pixels: the unit's origin inside the area is lrf_po = (lru_x * lru_sb_w,
+ * lru_y * lru_sb_h) superblocks with lru_sb_w = (unit_size << xdec) / 64, and its visible rect is
+ * vis_w = min(unit_size, ((frame_width - area_x) >> xdec) - lrf_po.x), vis_h likewise (rdo.rs:2651-2658;
+ * a floor shift, so an odd luma crop's last 4:2:0 chroma column is outside it).
+ *  1. None: rdo_loop_plane_error (rdo.rs:2027-2093) of lrf_in over the unit's superblocks (luma
+ *     cdef_dist_kernel 8x8, chroma sse_wxh, each times the 8x8 block's frame-absolute distortion_scale,
+ *     blocks inside the area's 8x8 grid only, the sum times dist_scale[p]).  Its rate is
+ *     count_lrf_switchable of the INCOMING filter, as the reference passes best_new_lrf (rdo.rs:2633-2638):
+ *     an Sgrproj incumbent charges None its own rate.  Taken if incoming_cost < 0 or cost < incoming_cost.
+ *  2. The integral image of lrf_in over vis (setup_integral_image, lrf.rs:529-627) in the area's scratch
+ *     copy: 4 real columns on the left unless the unit starts at the area's left edge, the last column
+ *     repeated on the right, real rows down to 2 above the unit (clamped to the area's row 0), the last row
+ *     repeated below.  All reads stay inside the area.
+ *  3. For each set of get_sgr_sets (all 16, or 1, 3, .. 15 with reduced_sets): sgrproj_solve
+ *     (lrf.rs:846-1096), sgrproj_stripe_filter over vis, rdo_loop_plane_error with the filtered pixels
+ *     inside vis and B200_LRF_WORK_FILL outside it, the rate sgr_bits + (4 << 3) + the signed subexp bits
+ *     of xqd against sgrproj_ref (context/frame_header.rs:14-45, ec.rs:639-773), compute_rd_cost; taken
+ *     on a strict `<`.
+ * The solve's sums are exact: every term is below 2^34 in magnitude and a 256x256 unit's total below
+ * 2^50, so the reference's f64 accumulation of i64 line sums equals one i64 total, and the rest of the
+ * solve runs the reference's f64 operations one for one; results are bit exact.
+ *
+ * lrf_in / src: HOST arrays of `planes` planes: the pass's lrf_input (the `out` of b200_cdef_rdo_dev, or the
+ * deblocked frame with CDEF off) and the input, covering at least the frame rounded up to 8 luma pixels.
+ * unit_size[p]: RestorationPlaneConfig::unit_size, whole superblocks (unit_size << dec a multiple of 64),
+ * 32..256.  d_imp_scales / dist_scale / lambda as b200_cdef_rdo_dev.  areas: HOST, as b200_cdef_rdo_dev.
+ * Outputs on the device, per item i: d_best[i] (the winner: the incoming filter when nothing beat it),
+ * d_cost[i] (its cost, the incoming cost when nothing improved), d_changed[i] = incoming.notequal(best)
+ * (lrf.rs:139-160).  Optional (NULL = not wanted): d_xqd[(i * 16 + set) * 2 + k], d_err[i * 17 + c] and
+ * d_cand_cost[i * 17 + c] with c = 0 for None and 1 + set for each set searched; other slots untouched.
+ * Rejected with B200_ERR_ARG before any launch, with nothing written: NULL pointers, a bpp that does not
+ * match bit_depth (8 / 10 / 12), planes other than 1 / 3, a layout other than 4:2:0 / 4:2:2 / 4:4:4, bad
+ * frame sizes, planes smaller than the frame's 8x8 blocks, a unit size that is not a power of two in
+ * 32..256 made of whole superblocks, an area outside the frame or larger than 4x4 superblocks, an item
+ * whose area or plane index is out of range or whose unit starts outside its area or its visible crop, an
+ * incoming record that is Wiener (the reference has no rate for it) or out of range, and a sgrproj_ref out
+ * of SGRPROJ_XQD_MIN..MAX.  n_items == 0 launches nothing. */
+/* The pixels of the reference's lrf_work outside each unit's visible rect: Plane::new's fill (v_frame
+ * 0.3.9, off disk upstream; restated as T::cast_from(128) and parity-unpinned). */
+#define B200_LRF_WORK_FILL 128
+typedef struct {
+  int32_t area;            /* index into areas */
+  int32_t plane;           /* 0..planes-1 */
+  int32_t lru_x, lru_y;    /* the unit inside the area, in units of this plane */
+  b200_lrf_unit incoming;  /* best_lrf of the unit on entry: None or Sgrproj */
+  uint32_t none_bits;      /* symbol_bits(0, lrf_switchable_cdf) */
+  double incoming_cost;    /* best_lrf_cost on entry; < 0 = none yet */
+  uint32_t sgr_bits;       /* symbol_bits(2, lrf_switchable_cdf) */
+  int8_t sgrproj_ref[2];   /* the plane's TileRestorationPlane::sgrproj_ref */
+  uint8_t pad_[2];
+} b200_lrf_search_item;    /* 48 B */
+int b200_lrf_search_dev(b200_ctx *ctx, const b200_plane *lrf_in, const b200_plane *src, int planes, int xdec,
+                        int ydec, int frame_width, int frame_height, int bit_depth, const int unit_size[3],
+                        int reduced_sets, const uint32_t *d_imp_scales, const uint32_t dist_scale[3],
+                        double lambda, const b200_cdef_rdo_area *areas, size_t n_areas,
+                        const b200_lrf_search_item *items, size_t n_items, b200_lrf_unit *d_best,
+                        double *d_cost, uint8_t *d_changed, int8_t *d_xqd, uint64_t *d_err,
+                        double *d_cand_cost);
+
 /* ------------------------------------------------------- intra prediction (predict.rs)
  * Boundary = rust::dispatch_predict_intra(mode, variant, dst, tx_size, bit_depth, ac, angle,
  * ief_params, edge_buf, cpu) (predict.rs:705-784; the asm wrappers, asm/x86/predict.rs:239-873,

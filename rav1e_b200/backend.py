@@ -112,6 +112,11 @@ assert DEBLOCK_MI_DTYPE.itemsize == 12 and DEBLOCK_ITEM_DTYPE.itemsize == 24 and
 LRF_UNIT_DTYPE = np.dtype([("type", "u1"), ("set", "u1"), ("xqd", "i1", (2,)), ("coeffs", "i1", (2, 3)),
                            ("pad_", "u1", (2,))])
 assert LRF_UNIT_DTYPE.itemsize == 12
+# b200_lrf_search_item (include/b200rdo.h)
+LRF_SEARCH_ITEM_DTYPE = np.dtype(
+    {"names": ["area", "plane", "lru_x", "lru_y", "incoming", "none_bits", "incoming_cost", "sgr_bits", "sgrproj_ref"],
+     "formats": ["<i4", "<i4", "<i4", "<i4", LRF_UNIT_DTYPE, "<u4", "<f8", "<u4", ("i1", (2,))],
+     "offsets": [0, 4, 8, 12, 16, 28, 32, 40, 44], "itemsize": 48})
 ME_RESULT_DTYPE = np.dtype(
     {"names": ["cost", "sad", "mv_row", "mv_col"],
      "formats": ["<u8", "<u4", "<i2", "<i2"], "offsets": [0, 8, 12, 14], "itemsize": 16})
@@ -267,6 +272,7 @@ def lib():
     L.b200_deblock_levels_dev.argtypes = [vp, vp, vp] + [i32] * 4 + [vp, i32, vp, sz, vp, vp]
     L.b200_deblock_filter_dev.argtypes = [vp, vp, vp] + [i32] * 4 + [vp, vp, vp, i32, vp, sz]
     L.b200_lrf_filter_dev.argtypes = [vp, vp, vp, vp] + [i32] * 7 + [vp, vp]
+    L.b200_lrf_search_dev.argtypes = [vp, vp, vp] + [i32] * 6 + [vp, i32, vp, vp, C.c_double, vp, sz, vp, sz] + [vp] * 6
     _LIB = L
     return L
 
@@ -597,6 +603,24 @@ class Context:
         self.check(self.L.b200_lrf_filter_dev(self.h, C.addressof(c_), C.addressof(d_), C.addressof(o), n, xdec, ydec,
                                               frame_w, frame_h, bit_depth, int(enable_cdef), C.addressof(us),
                                               C.addressof(ptrs)))
+
+    def lrf_search_dev(self, lrf_in, src, xdec, ydec, frame_w, frame_h, bit_depth, unit_size, reduced_sets,
+                       d_imp_scales, dist_scale, lam, areas, items, d_best, d_cost, d_changed, d_xqd=None, d_err=None,
+                       d_cand_cost=None):
+        """lrf_in / src: lists of 1 or 3 Plane; areas: [(sbx, sby, sb_w, sb_h), ...]; items: a host
+        LRF_SEARCH_ITEM_DTYPE array; outputs on the device: d_best (LRF_UNIT_DTYPE per item), d_cost (f64),
+        d_changed (u8), optional d_xqd (items x 16 x 2 i8), d_err (items x 17 u64), d_cand_cost (items x 17
+        f64) (include/b200rdo.h)."""
+        i_, s_ = self._plane_array(lrf_in), self._plane_array(src)
+        ar = np.ascontiguousarray(np.asarray(areas, np.int32).reshape(-1, 4))
+        it = np.ascontiguousarray(np.asarray(items, LRF_SEARCH_ITEM_DTYPE).reshape(-1))
+        us = (C.c_int * 3)(*[int(v) for v in unit_size], *([0] * (3 - len(unit_size))))
+        ds = (C.c_uint32 * 3)(*[int(v) for v in dist_scale])
+        self.check(self.L.b200_lrf_search_dev(
+            self.h, C.addressof(i_), C.addressof(s_), len(lrf_in), xdec, ydec, frame_w, frame_h, bit_depth,
+            C.addressof(us), int(reduced_sets), _dev_ptr(d_imp_scales), C.addressof(ds), float(lam), ar.ctypes.data,
+            len(ar), it.ctypes.data, len(it), _dev_ptr(d_best), _dev_ptr(d_cost), _dev_ptr(d_changed),
+            _dev_ptr(d_xqd), _dev_ptr(d_err), _dev_ptr(d_cand_cost)))
 
     # ---- intra prediction
     def predict_intra_dev(self, d_edges, d_items, n, d_ac, w, h, bit_depth, plane_w, plane_h, d_out):

@@ -21,6 +21,7 @@
 
 #include "common.cuh"
 #include "host_stage.cuh"
+#include "lrf_dev.cuh"
 
 namespace {
 
@@ -33,11 +34,6 @@ constexpr int kSW = kTW + 6;            // staged columns: the span plus 3 left 
 constexpr int kAbRows = 64 + 2;         // radius-1 a / b rows: -1 .. 64
 constexpr int kAbCols = kTW + 2;        // a / b columns: -1 .. kTW
 
-// SGRPROJ_PARAMS_S (lrf.rs:56-73): s for radius 2, s for radius 1
-__constant__ uint16_t kSgrS[16][2] = {{140, 3236}, {112, 2158}, {93, 1618}, {80, 1438}, {70, 1295}, {58, 1177},
-                                      {47, 1079},  {37, 996},   {30, 925},  {25, 863},  {0, 2589},  {0, 1618},
-                                      {0, 1177},   {0, 925},    {56, 0},    {22, 0}};
-
 struct LrfArgs {
   PlaneView cdef[3], deb[3], out[3];
   int cw[3], ch[3], yd[3];       // crop and vertical decimation per plane
@@ -48,19 +44,6 @@ struct LrfArgs {
   const b200_lrf_unit *units[3];
   int bit_depth, enable_cdef;
 };
-
-// sgrproj_sum_finish (lrf.rs:344-362), u32 arithmetic as the reference
-__device__ __forceinline__ void sum_finish(uint32_t ssq, uint32_t sum, uint32_t n, uint32_t one_over_n, uint32_t s,
-                                           int bdm8, uint32_t &ra, uint32_t &rb) {
-  const uint32_t scaled_ssq = (ssq + ((1u << (2 * bdm8)) >> 1)) >> (2 * bdm8);
-  const uint32_t scaled_sum = (sum + ((1u << bdm8) >> 1)) >> bdm8;
-  const uint32_t t0 = scaled_ssq * n, t1 = scaled_sum * scaled_sum;
-  const uint32_t p = t0 > t1 ? t0 - t1 : 0;
-  const uint32_t z = (p * s + (1u << 19)) >> 20;
-  const uint32_t a = z >= 255 ? 256 : z == 0 ? 1 : ((z << 8) + z / 2) / (z + 1);
-  ra = a;
-  rb = ((256 - a) * sum * one_over_n + (1u << 11)) >> 12;
-}
 
 template <typename T>
 __global__ void __launch_bounds__(kThreads) lrf_filter_kernel(const LrfArgs a) {
@@ -177,13 +160,13 @@ __global__ void __launch_bounds__(kThreads) lrf_filter_kernel(const LrfArgs a) {
       const uint32_t px = sp[y + 3][lane + 3];
       // sgrproj_box_f_r2 (lrf.rs:300-342): even rows weigh rows y - 1 and y + 1, odd rows their own
       const int j = (y + 1) >> 1;
-      uint32_t av = 5 * (u.ab.A[j][lane] + u.ab.A[j][lane + 2]) + 6 * u.ab.A[j][lane + 1];
-      uint32_t bv = 5 * (u.ab.B[j][lane] + u.ab.B[j][lane + 2]) + 6 * u.ab.B[j][lane + 1];
+      uint32_t av = r2_row(u.ab.A[j], lane);
+      uint32_t bv = r2_row(u.ab.B[j], lane);
       if (y & 1) {
         f2[k] = (av * px + bv + (1u << 7)) >> 8;
       } else {
-        av += 5 * (u.ab.A[j + 1][lane] + u.ab.A[j + 1][lane + 2]) + 6 * u.ab.A[j + 1][lane + 1];
-        bv += 5 * (u.ab.B[j + 1][lane] + u.ab.B[j + 1][lane + 2]) + 6 * u.ab.B[j + 1][lane + 1];
+        av += r2_row(u.ab.A[j + 1], lane);
+        bv += r2_row(u.ab.B[j + 1], lane);
         f2[k] = (av * px + bv + (1u << 8)) >> 9;
       }
     }
@@ -222,12 +205,7 @@ __global__ void __launch_bounds__(kThreads) lrf_filter_kernel(const LrfArgs a) {
     const uint32_t px = sp[y + 3][lane + 3];
     uint32_t f1 = px << 4;
     if (s1) {  // sgrproj_box_f_r1 (lrf.rs:266-291)
-      const uint32_t(*A)[kAbCols] = u.ab.A, (*B)[kAbCols] = u.ab.B;
-      const int l = lane;
-      const uint32_t av = 3 * (A[y][l] + A[y + 2][l] + A[y][l + 2] + A[y + 2][l + 2]) +
-                          4 * (A[y + 1][l] + A[y][l + 1] + A[y + 1][l + 1] + A[y + 2][l + 1] + A[y + 1][l + 2]);
-      const uint32_t bv = 3 * (B[y][l] + B[y + 2][l] + B[y][l + 2] + B[y + 2][l + 2]) +
-                          4 * (B[y + 1][l] + B[y][l + 1] + B[y + 1][l + 1] + B[y + 2][l + 1] + B[y + 1][l + 2]);
+      const uint32_t av = r1_weigh(u.ab.A, y, lane), bv = r1_weigh(u.ab.B, y, lane);
       f1 = (av * px + bv + (1u << 8)) >> 9;
     }
     // apply_filter (lrf.rs:796-815)
