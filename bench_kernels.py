@@ -82,7 +82,7 @@ def card():
     return d
 
 
-def emit(name, units, unit_name, ms, bytes_per_unit, note="", cpu=None, extra=None):
+def emit(name, units, unit_name, ms, bytes_per_unit, note="", cpu=None, extra=None, cpu_threads=None):
     gbs = units * bytes_per_unit / (ms * 1e-3) / 1e9
     d = {"kernel": name, "units_per_launch": units, "unit": unit_name, "launch_ms": ms,
          "units_per_s": units / (ms * 1e-3), "algorithmic_bytes_per_unit": bytes_per_unit,
@@ -90,7 +90,7 @@ def emit(name, units, unit_name, ms, bytes_per_unit, note="", cpu=None, extra=No
     d.update(extra or {})
     if cpu is not None:
         d["cpu_port_units_per_s"] = cpu
-        d["cpu_threads"] = O.host_threads()
+        d["cpu_threads"] = cpu_threads if cpu_threads is not None else O.host_threads()
         d["gpu_over_cpu"] = d["units_per_s"] / cpu
     print(json.dumps(d))
 
@@ -768,6 +768,52 @@ def lrf_search(ctx):
             ctx.plane_free(p)
 
 
+def loop_decision(ctx):
+    """b200_loop_decision_dev over a whole 1080p 4:2:0 frame at 8 and 10 bit (seeded smooth content plus noise,
+    30% of the 8x8 blocks skipped, 20% of the units lru_skip), every area in one call, for the unit
+    configurations of the search leg with the Full and Reduced set lists.  The time includes the per-stage status
+    reads.  Next to it, orc_loop_decision on one host thread on the same inputs, and a check of every output."""
+    from tests.test_oracle_loop_decision import case, run
+    W, H = 1920, 1080
+    for bd in (8, 10):
+        for uy in (64, 128, 256):
+            fx = case(100 + bd + uy, "420", bd, W, H, (uy, uy >> 1, uy >> 1), lam=500.0)
+            d_rec = [ctx.plane_from_host(a, 8) for a in fx["rec"]]
+            d_src = [ctx.plane_from_host(a, 8) for a in fx["src"]]
+            d_work = [ctx.plane_from_host(np.zeros_like(a), 8) for a in fx["rec"]]
+            d_skip = dev(fx["skip8"].reshape(-1))
+            d_imp = dev(fx["imp"].reshape(-1))
+            n, nu = len(fx["areas"]), len(fx["units"])
+            # the oracle wrapper's sentinels: areas that run no stage leave their slots and units untouched
+            d_best, d_unit = dev(np.full(16 * n, 127, np.int8)), dev(np.full(12 * nu, 0xEE, np.uint8))
+            d_ucost, d_wr = dev(np.full(nu, np.nan)), dev(np.full(nu, 7, np.uint8))
+            for reduced in (0, 1):
+                fx["reduced"] = bool(reduced)
+                got = {}
+
+                def call():
+                    got["stages"] = ctx.loop_decision_dev(
+                        d_rec, d_src, d_work, 1, 1, W, H, bd, 1, fx["damping"], fx["cdef_bits"], fx["ystr"],
+                        fx["uvstr"], d_skip, 1, fx["unit_size"], reduced, d_imp, fx["dist_scale"], fx["lam"],
+                        fx["areas"], fx["units"], fx["sb_unit"], d_best, d_unit, d_ucost, d_wr)
+                ms = timed(call)
+                want = run(fx)
+                same = bool(got["stages"] == want[0] and (d_best.cpu().numpy().view(np.int8) == want[1][:16 * n]).all() and
+                            (d_unit.cpu().numpy().view(np.uint8) == want[2].view(np.uint8)).all() and
+                            (d_ucost.cpu().numpy().view(np.uint64) == want[3].view(np.uint64)).all() and
+                            (d_wr.cpu().numpy() == want[4]).all())
+                assert same, f"loop_decision {uy} reduced={reduced} {bd}-bit disagrees with the oracle"
+                cpu = cpu_rate(lambda: run(fx), 1)
+                extra = {"bit_depth": bd, "unit_size": list(fx["unit_size"]), "sets": "reduced" if reduced else "full",
+                         "areas": n, "units": nu, "stages": got["stages"], "same_as_oracle": same,
+                         "library": os.path.basename(B.LIB_PATH)}
+                emit(f"loop_decision_dev units {uy}/{uy >> 1} {'reduced' if reduced else 'full'} sets {bd}-bit 4:2:0",
+                     1, "frames", ms, 0, "1080p seeded, every area in one call, per-stage status reads included",
+                     cpu=cpu, extra=extra, cpu_threads=1)  # orc_loop_decision runs on one thread
+            for p in d_rec + d_src + d_work:
+                ctx.plane_free(p)
+
+
 def main():
     torch.cuda.set_device(0)
     stream = torch.cuda.Stream()
@@ -797,6 +843,9 @@ def main():
         return
     if "--lrf-search" in sys.argv[1:]:
         lrf_search(ctx)
+        return
+    if "--loop-decision" in sys.argv[1:]:
+        loop_decision(ctx)
         return
     rng = np.random.default_rng(0)
     W, H, PAD = 1920, 1080, 96

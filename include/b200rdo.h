@@ -915,6 +915,91 @@ int b200_lrf_search_dev(b200_ctx *ctx, const b200_plane *lrf_in, const b200_plan
                         double *d_cost, uint8_t *d_changed, int8_t *d_xqd, uint64_t *d_err,
                         double *d_cand_cost);
 
+/* rdo_loop_decision (rdo.rs:2104-2745) from the point after its optional deblock, for a HOST list of
+ * loop-restoration areas in one call: the CDEF analysis, then the pass loop of CDEF stages (C) and
+ * restoration stages (L), C, L, C, L, .., per area until a stage changes nothing.  Unlike its neighbours this
+ * call SYNCHRONISES the context's stream: the number of stages depends on the data, so after every stage it
+ * reads back one small status record (the count of areas still changing); nothing else comes back.  Areas
+ * are independent, as in the reference (each has its own scratch copy).
+ *
+ * Per area: it has CDEF work when enable_cdef and some 8x8 block of it is not skipped (!cdef_skip_all), and
+ * restoration work (lrf_work) when enable_restoration and some unit of it has `search` set.  An area with
+ * neither gets no stage (rdo.rs:2267).  A C stage counts as changed on the first pass whatever it does
+ * (cdef_change starts true) and afterwards when some superblock's index changed; without CDEF work it does
+ * nothing.  An L stage counts as changed when some unit's filter changed; without lrf_work it does nothing
+ * and is unchanged.  An area stops after its first unchanged stage; its stage count includes that stage.
+ *  C: every superblock that is not CDEF-skipped, in raster order, tries every index 0 .. 1 << cdef_bits as
+ *     b200_cdef_rdo_dev does, except for the restoration terms of each plane p whose map entry u =
+ *     sb_unit[(area * 16 + sby * 4 + sbx) * 3 + p] is not -1, when the area has lrf_work:
+ *     - the rate adds count_lrf_switchable of unit u's current filter: none_bits for None, sgr_bits +
+ *       (4 << 3) + the signed subexp bits of xqd against sgrproj_ref for Sgrproj (rdo.rs:2446-2506);
+ *     - for Sgrproj, the plane's distortion is measured after the self-guided filter (rdo.rs:2458-2500):
+ *       the integral image of the CDEF working copy over the superblock's visible rect with crop = stripe
+ *       = vis (4 real columns on the left unless the superblock is in the area's column 0, 2 real rows
+ *       above clamped to the area's row 0, nothing real right or below), sgrproj_stripe_filter with the
+ *       unit's set and xqd, then rdo_loop_plane_error with the filtered pixels inside vis and
+ *       B200_LRF_WORK_FILL outside it.  Those left / upper pixels are THIS pass's winners of the left, upper
+ *       and upper-left superblocks (rdo.rs:2554-2564 re-filters every winner in raster order), so the
+ *       device runs each C stage one anti-diagonal of superblocks at a time.
+ *     Without lrf_work the rate is 0 and the distortion is the CDEF output's (the no-LRU branch).  The
+ *     first minimum wins; the winner is filtered into the working copy.
+ *  L: b200_lrf_search_dev's computation over the units with `search` set, reading the working copy (rec for
+ *     an area without CDEF work), with the incumbent filter and best_lrf_cost carried from the previous L
+ *     stage (None and -1 on the first).
+ *
+ * rec: HOST array of `planes` planes, the deblocked reconstruction (b200_deblock_filter_dev's `out` over the
+ * same areas, or the reconstruction when deblocking is off).  src: the input.  work: the caller's CDEF
+ * working copy (the reference's cdef_work), aliasing neither rec nor src; every area that runs a stage gets
+ * a copy of rec over its scratch rect first, and holds afterwards the last C stage's output there (rec
+ * itself for an area without CDEF work).  Nothing outside those rects is written.  Planes cover at least
+ * the frame rounded up to 8 luma pixels.  enable_cdef / damping / cdef_bits / strengths / d_skip8 as
+ * b200_cdef_rdo_dev (the strengths are not read with enable_cdef == 0); enable_restoration / unit_size /
+ * reduced_sets as b200_lrf_search_dev (unit_size is not read with enable_restoration == 0);
+ * d_imp_scales / dist_scale / lambda as both.
+ *
+ * units: HOST array of n_units records, one per restoration unit of an area and plane the caller tracks
+ * (TileRestorationState's units, which stay with the caller); sb_unit: HOST, n_areas * 16 * 3 entries,
+ * each an index into units or -1, mirroring restoration_unit_offset(base_sbo, loop_sbo, false) for every
+ * superblock slot of every area (entries of slots outside an area are not read).
+ * Outputs on the device: d_best_index[slot] (area * 16 + sby * 4 + sbx): the final index, -1 for
+ * CDEF-skipped superblocks and every superblock of an area without CDEF work (set_cdef reads it); per unit
+ * d_unit[u], d_unit_cost[u] (best_lrf_cost) and d_written[u] = 1 when the unit's filter changed at some
+ * stage of the call, so the caller can apply rdo.rs:2730-2741's conditional `ru.filter = ..` exactly.
+ * Optional (NULL = not wanted): d_err / d_cost of the LAST C stage that evaluated a superblock, laid out as
+ * b200_cdef_rdo_dev's.  Slots and units of areas that run no stage, and slots outside the areas, are not
+ * written.  *stages: the number of stages of the longest area (0 when no area runs one), or -1 when an
+ * area was still changing after B200_LOOP_MAX_STAGES stages, where the call stops.
+ * Rejected with B200_ERR_ARG before any launch, with nothing written: a NULL ctx / rec / src / work /
+ * dist_scale / stages / d_best_index, or NULL unit outputs with n_units > 0; a bpp that does not match
+ * bit_depth (8 / 10 / 12); planes other than 1 / 3; a layout other than 4:2:0 / 4:2:2 / 4:4:4; bad frame
+ * sizes; planes smaller than the frame's 8x8 blocks; work aliasing rec or src; with enable_cdef, NULL
+ * strengths, cdef_bits outside 0..3, a used strength above 63 or damping outside 3..6; with
+ * enable_restoration, a NULL unit_size or a unit size as b200_lrf_search_dev rejects it; areas outside
+ * the frame, larger than 4x4 superblocks or overlapping each other; n_areas > 0 with NULL areas / sb_unit;
+ * n_units > 0 with NULL units; a unit whose area or plane is out of range, which starts outside its area
+ * or its visible crop, or whose sgrproj_ref is out of SGRPROJ_XQD_MIN..MAX; a map entry outside -1 ..
+ * n_units - 1 or naming a unit of another area or plane.  n_areas == 0 launches nothing. */
+#define B200_LOOP_MAX_STAGES 64
+typedef struct {
+  int32_t area;            /* index into areas */
+  int32_t plane;           /* 0..planes-1 */
+  int32_t lru_x, lru_y;    /* the unit inside the area, in units of this plane */
+  uint32_t none_bits;      /* symbol_bits(0, lrf_switchable_cdf) */
+  uint32_t sgr_bits;       /* symbol_bits(2, lrf_switchable_cdf) */
+  int8_t sgrproj_ref[2];   /* the plane's TileRestorationPlane::sgrproj_ref */
+  uint8_t search;          /* !lru_skip && has_restoration_unit(.., false) (rdo.rs:2212-2263, 2593-2611) */
+  uint8_t pad_;
+} b200_loop_unit;          /* 28 B */
+int b200_loop_decision_dev(b200_ctx *ctx, const b200_plane *rec, const b200_plane *src, const b200_plane *work,
+                           int planes, int xdec, int ydec, int frame_width, int frame_height, int bit_depth,
+                           int enable_cdef, int damping, int cdef_bits, const uint8_t y_strengths[8],
+                           const uint8_t uv_strengths[8], const uint8_t *d_skip8, int enable_restoration,
+                           const int unit_size[3], int reduced_sets, const uint32_t *d_imp_scales,
+                           const uint32_t dist_scale[3], double lambda, const b200_cdef_rdo_area *areas,
+                           size_t n_areas, const b200_loop_unit *units, size_t n_units, const int32_t *sb_unit,
+                           int8_t *d_best_index, b200_lrf_unit *d_unit, double *d_unit_cost, uint8_t *d_written,
+                           uint64_t *d_err, double *d_cost, int *stages);
+
 /* ------------------------------------------------------- intra prediction (predict.rs)
  * Boundary = rust::dispatch_predict_intra(mode, variant, dst, tx_size, bit_depth, ac, angle,
  * ief_params, edge_buf, cpu) (predict.rs:705-784; the asm wrappers, asm/x86/predict.rs:239-873,

@@ -117,6 +117,11 @@ LRF_SEARCH_ITEM_DTYPE = np.dtype(
     {"names": ["area", "plane", "lru_x", "lru_y", "incoming", "none_bits", "incoming_cost", "sgr_bits", "sgrproj_ref"],
      "formats": ["<i4", "<i4", "<i4", "<i4", LRF_UNIT_DTYPE, "<u4", "<f8", "<u4", ("i1", (2,))],
      "offsets": [0, 4, 8, 12, 16, 28, 32, 40, 44], "itemsize": 48})
+# b200_loop_unit (include/b200rdo.h)
+LOOP_UNIT_DTYPE = np.dtype([("area", "<i4"), ("plane", "<i4"), ("lru_x", "<i4"), ("lru_y", "<i4"),
+                            ("none_bits", "<u4"), ("sgr_bits", "<u4"), ("sgrproj_ref", "i1", (2,)), ("search", "u1"),
+                            ("pad_", "u1")])
+assert LOOP_UNIT_DTYPE.itemsize == 28
 ME_RESULT_DTYPE = np.dtype(
     {"names": ["cost", "sad", "mv_row", "mv_col"],
      "formats": ["<u8", "<u4", "<i2", "<i2"], "offsets": [0, 8, 12, 14], "itemsize": 16})
@@ -272,6 +277,8 @@ def lib():
     L.b200_deblock_levels_dev.argtypes = [vp, vp, vp] + [i32] * 4 + [vp, i32, vp, sz, vp, vp]
     L.b200_deblock_filter_dev.argtypes = [vp, vp, vp] + [i32] * 4 + [vp, vp, vp, i32, vp, sz]
     L.b200_lrf_filter_dev.argtypes = [vp, vp, vp, vp] + [i32] * 7 + [vp, vp]
+    L.b200_loop_decision_dev.argtypes = [vp, vp, vp, vp] + [i32] * 9 + [vp, vp, vp, i32, vp, i32, vp, vp,
+                                                                        C.c_double, vp, sz, vp, sz] + [vp] * 8
     L.b200_lrf_search_dev.argtypes = [vp, vp, vp] + [i32] * 6 + [vp, i32, vp, vp, C.c_double, vp, sz, vp, sz] + [vp] * 6
     _LIB = L
     return L
@@ -621,6 +628,33 @@ class Context:
             C.addressof(us), int(reduced_sets), _dev_ptr(d_imp_scales), C.addressof(ds), float(lam), ar.ctypes.data,
             len(ar), it.ctypes.data, len(it), _dev_ptr(d_best), _dev_ptr(d_cost), _dev_ptr(d_changed),
             _dev_ptr(d_xqd), _dev_ptr(d_err), _dev_ptr(d_cand_cost)))
+
+    def loop_decision_dev(self, rec, src, work, xdec, ydec, frame_w, frame_h, bit_depth, enable_cdef, damping,
+                          cdef_bits, y_strengths, uv_strengths, d_skip8, enable_restoration, unit_size, reduced_sets,
+                          d_imp_scales, dist_scale, lam, areas, units, sb_unit, d_best_index, d_unit, d_unit_cost,
+                          d_written, d_err=None, d_cost=None):
+        """rdo_loop_decision's pass loop (include/b200rdo.h).  rec / src / work: lists of 1 or 3 Plane; areas:
+        [(sbx, sby, sb_w, sb_h), ...]; units: a host LOOP_UNIT_DTYPE array; sb_unit: n_areas x 16 x 3 int32 unit
+        indices or -1; outputs on the device: d_best_index (n_areas * 16 i8), d_unit (LRF_UNIT_DTYPE per unit),
+        d_unit_cost (f64), d_written (u8), optional d_err / d_cost (n_areas * 16 * 8).  Synchronises the
+        stream; returns the stage count (-1: still changing after B200_LOOP_MAX_STAGES)."""
+        r, s_, w = self._plane_array(rec), self._plane_array(src), self._plane_array(work)
+        ar = np.ascontiguousarray(np.asarray(areas, np.int32).reshape(-1, 4))
+        un = np.ascontiguousarray(np.asarray(units, LOOP_UNIT_DTYPE).reshape(-1))
+        mp = np.ascontiguousarray(np.asarray(sb_unit, np.int32).reshape(-1))
+        ys = (C.c_uint8 * 8)(*[int(v) for v in y_strengths])
+        us_ = (C.c_uint8 * 8)(*[int(v) for v in uv_strengths])
+        usz = (C.c_int * 3)(*[int(v) for v in unit_size], *([0] * (3 - len(unit_size))))
+        ds = (C.c_uint32 * 3)(*[int(v) for v in dist_scale])
+        stages = C.c_int(0)
+        self.check(self.L.b200_loop_decision_dev(
+            self.h, C.addressof(r), C.addressof(s_), C.addressof(w), len(rec), xdec, ydec, frame_w, frame_h,
+            bit_depth, int(enable_cdef), damping, cdef_bits, C.addressof(ys), C.addressof(us_), _dev_ptr(d_skip8),
+            int(enable_restoration), C.addressof(usz), int(reduced_sets), _dev_ptr(d_imp_scales), C.addressof(ds),
+            float(lam), ar.ctypes.data, len(ar), un.ctypes.data if len(un) else None, len(un), mp.ctypes.data,
+            _dev_ptr(d_best_index), _dev_ptr(d_unit), _dev_ptr(d_unit_cost), _dev_ptr(d_written), _dev_ptr(d_err),
+            _dev_ptr(d_cost), C.byref(stages)))
+        return stages.value
 
     # ---- intra prediction
     def predict_intra_dev(self, d_edges, d_items, n, d_ac, w, h, bit_depth, plane_w, plane_h, d_out):
