@@ -814,6 +814,50 @@ def loop_decision(ctx):
                 ctx.plane_free(p)
 
 
+def segmentation(ctx):
+    """b200_segmentation_optimize_dev on a 1080p score map (240 x 135 importance blocks, lognormal scores) at 8 and
+    10 bit, and b200_select_segment_dev over every block of the 1080p frame at 8x8 and at 64x64 with each level.
+    Algorithmic bytes: the score map once (optimize); per block its distortion and activity entries, the item
+    and the outputs (select).  Next to each, the oracle on one host thread on the same inputs, and a check of
+    every output against it.  A call is tens of microseconds, so each line times 500 back-to-back calls."""
+    from tests.test_oracle_segmentation import AC_Q, oracle_optimize, oracle_select, scale_maps, score_maps
+    from tests.test_segmentation_gpu import frame_items
+    W, H = 1920, 1080
+    w, h = (W + 7) // 8, (H + 7) // 8
+    name, scores, mw, mh = score_maps()[0]
+    assert (mw, mh) == (w, h), name
+    d_sc, d_rec = dev(scores), dev(np.zeros(240, np.uint8))
+    lib = os.path.basename(B.LIB_PATH)
+    for bd in (8, 10):
+        ms = timed(lambda: ctx.segmentation_optimize_dev(d_sc, w, h, 120, bd, AC_Q[bd], 1, None, d_rec), reps=500)
+        want = oracle_optimize(scores, w, h, 120, bd, 1, None)
+        same = d_rec.cpu().numpy().tobytes() == want.tobytes()
+        assert same, f"segmentation_optimize {bd}-bit disagrees with the oracle"
+        cpu = cpu_rate(lambda: oracle_optimize(scores, w, h, 120, bd, 1, None), 1)
+        emit(f"segmentation_optimize_dev 1080p map {bd}-bit", 1, "frames", ms, 4 * w * h,
+             "240x135 lognormal scores, base_q_idx 120; launch_ms includes the histogram clear", cpu=cpu,
+             extra={"bit_depth": bd, "segments": int(want["max_segment"][0]) + 1, "same_as_oracle": same,
+                    "library": lib}, cpu_threads=1)
+    d, a = scale_maps(w, h, seed=13)
+    d_d, d_a = dev(d), dev(a)
+    rec = d_rec.cpu().numpy().view(B.SEGMENTATION_DTYPE)  # the 10-bit record
+    for bs, label, imp in ((3, "8x8", 1), (12, "64x64", 64)):  # imp: importance blocks per block
+        items = frame_items(W, H, bs)
+        n = len(items)
+        d_it, d_sidx, d_scale = dev(items), dev(np.zeros(2 * n, np.uint8)), dev(np.zeros(n, np.uint32))
+        for level, lname in ((1, "simple"), (2, "complex"), (3, "full")):
+            ms = timed(lambda: ctx.select_segment_dev(d_it, n, d_d, d_a, w, h, 0, level, d_rec, d_sidx, d_scale),
+                       reps=500)
+            want, want_scale = oracle_select(items, d, a, w, h, 0, level, rec)
+            same = bool((d_sidx.cpu().numpy().reshape(-1, 2) == want).all() and
+                        (d_scale.cpu().numpy().view(np.uint32) == want_scale).all())
+            assert same, f"select_segment {label} {lname} disagrees with the oracle"
+            cpu = cpu_rate(lambda: oracle_select(items, d, a, w, h, 0, level, rec), n)
+            emit(f"select_segment_dev 1080p {label} blocks {lname}", n, "blocks", ms, 8 * imp + 8 + 2 + 4,
+                 "every block of the frame, 1/7 skipped; bytes: distortion + activity entries, item, outputs",
+                 cpu=cpu, extra={"items": n, "same_as_oracle": same, "library": lib}, cpu_threads=1)
+
+
 def main():
     torch.cuda.set_device(0)
     stream = torch.cuda.Stream()
@@ -846,6 +890,9 @@ def main():
         return
     if "--loop-decision" in sys.argv[1:]:
         loop_decision(ctx)
+        return
+    if "--segmentation" in sys.argv[1:]:
+        segmentation(ctx)
         return
     rng = np.random.default_rng(0)
     W, H, PAD = 1920, 1080, 96

@@ -569,6 +569,84 @@ int b200_temporal_scores_dev(b200_ctx *ctx, size_t w_imp, size_t h_imp, uint32_t
                              const uint32_t *d_activity, uint32_t *d_spatiotemporal,
                              int64_t *d_log_isqrt_mean_scale, uint32_t *d_scale4x4, size_t scale4x4_stride);
 
+/* ---------------------------------------------------------------- segmentation (segmentation.rs, rdo.rs)
+ * rav1e's adaptive quantization.  A frame step, segmentation_optimize (segmentation.rs:23-160, called at
+ * encoder.rs:3776-3779 after get_initial_segmentation), fits k-means (util/kmeans.rs, k = 3..8) to the
+ * binary logarithms of the frame's spatiotemporal scores and turns the centroids into per-segment q-index
+ * deltas and distortion thresholds; a block step, select_segment (segmentation.rs:163-196, called per skip
+ * choice at rdo.rs:855-861), places a block's spatiotemporal_scale (rdo.rs:464-504) among those thresholds.
+ * Both read and write device memory only; results are bit-identical to the reference.
+ *
+ * b200_segmentation mirrors SegmentationState (encoder.rs:550-562) field for field (bools as 0 / 1,
+ * SegLvl::SEG_LVL_ALT_Q = feature 0, threshold[] = Q14 DistortionScale) and adds:
+ *   qidx[s]  get_qidx (encoder.rs:1383-1394) of segment s: clamp(base_q_idx + data[s][0], 0, 255) where
+ *            features[s][0] is set (the i16 sum wraps as in a release build), else base_q_idx;
+ *   status   0, or where the reference panics: 1 = update_data == 0 and no segment has ALT_Q set with
+ *            data >= 1 - base_q_idx (segmentation.rs:52); 2 = update_data == 0 and the previous
+ *            max_segment > 7 (update_threshold's slice).  With a non-zero status the record holds the
+ *            previous state with enabled / update_map / update_data set and qidx filled; select_segment
+ *            treats every item as invalid. */
+typedef struct {
+  uint8_t enabled, update_data, update_map, preskip;
+  uint8_t last_active_segid, min_segment, max_segment, pad_;
+  uint8_t features[8][8]; /* [segment][SegLvl] */
+  int16_t data[8][8];     /* [segment][SegLvl] */
+  uint32_t threshold[7];  /* DistortionScale, Q14 */
+  uint8_t qidx[8];
+  int32_t status;
+} b200_segmentation; /* 240 B */
+/* segmentation_optimize for one frame.  d_spatiotemporal: the w_imp x h_imp score map that
+ * b200_temporal_scores_dev leaves (either form; w_imp = w_in_b / 2 on the ceil grid, as CodedFrameData),
+ * read only when update_data is 1.  ac_q: HOST copy of the caller's 256-entry ac_qlookup table for
+ * bit_depth (ac_qlookup_Q3 / _10_ / _12_, quantize/tables.rs); the library holds no quantizer tables.
+ * update_data = (primary_ref_frame == PRIMARY_REF_NONE).  d_prev: the previous state
+ * (get_initial_segmentation: the primary reference's record) or NULL for SegmentationState::default();
+ * it may equal d_out.  update_data 0: min_segment search and update_threshold with the previous
+ * max_segment, preskip / last_active_segid kept; 1: the k-means fit, then preskip / last_active_segid over
+ * all eight segments (entries past the chosen k keep the previous state's values, as in the reference).
+ * Thresholds use ac_q(base, data as i8): a delta outside -128..127 wraps there (not in data or qidx),
+ * and the thresholds then need not be monotone (see b200_select_segment_dev).
+ * Rejected with B200_ERR_ARG before anything is enqueued: NULL ctx / ac_q / d_out, NULL d_spatiotemporal
+ * with update_data 1, a bit depth other than 8 / 10 / 12, base_q_idx outside 0..255, update_data not 0 / 1,
+ * a map size of 0 or w_imp * h_imp >= 2^30, and a table with a zero or that is not strictly increasing
+ * (select_qi's binary search needs it).  With update_data 1: a histogram clear (cudaMemsetAsync) and two
+ * launches (the histogram, one 512-thread CTA); otherwise one launch.  Context scratch holds the histogram
+ * and its prefix sums (786 KB). */
+int b200_segmentation_optimize_dev(b200_ctx *ctx, const uint32_t *d_spatiotemporal, size_t w_imp, size_t h_imp,
+                                   int base_q_idx, int bit_depth, const uint16_t *ac_q, int update_data,
+                                   const b200_segmentation *d_prev, b200_segmentation *d_out);
+/* select_segment for a batch of blocks, each with its skip choice.  Per item: skip gives 0..=0; level Full
+ * gives min_segment..=max_segment; otherwise spatiotemporal_scale of the block (x0 = x >> 3,
+ * x1 = min(x0 + max(w >> 3, 1), w_imp), likewise y; the u64 sum of distortion x activity over at most
+ * MAX_SB_IN_IMP_B = 16 columns per row, wrapping; (sum + den / 2) / den with den = (x1 - x0)(y1 - y0) << 14,
+ * truncated to u32), its segment by segment_idx_from_distortion, raised to min_segment; Complex then gives
+ * sidx..=min(max_segment, sidx + 1), Simple sidx..=sidx.  segment_idx_from_distortion is
+ * threshold.partition_point(|t| s < t), restated as the branchless binary search of Rust 1.83's
+ * core::slice::binary_search_by (the reference's MSRV; the form since Rust 1.82): for monotone thresholds it
+ * has the one answer any search has; for the non-monotone ones an i8-wrapped delta can produce it follows
+ * that probe order.
+ * d_scales / d_activity: the distortion and activity scale maps (w_imp x h_imp; d_activity NULL = 1 << 14
+ * everywhere).  scales_off != 0: the block scale is DistortionScale::default() (rdo.rs:467-469: temporal RDO
+ * off and tune not Psychovisual); the maps are then not read and may be NULL.  level: SegmentationLevel
+ * discriminant 1 Simple, 2 Complex, 3 Full.  d_seg: the record of b200_segmentation_optimize_dev.
+ * d_sidx: nitems x 2 (sidx_lo, sidx_hi); d_scale (may be NULL): the block's Q14 spatiotemporal_scale
+ * (computed for every valid item, whatever its skip and the level).  Rejected with B200_ERR_ARG before any
+ * launch: NULL ctx / d_seg / d_sidx, NULL d_items with nitems > 0, NULL d_scales unless scales_off, a level
+ * outside 1..3, a map size of 0 or w_imp * h_imp >= 2^30.  An invalid item gets {255, 255} in d_sidx and
+ * UINT32_MAX in d_scale, and nothing is read for it: bsize >= 22, x or y negative or not a multiple of 4,
+ * x >> 3 >= w_imp or y >> 3 >= h_imp; so does every item when the record's status is non-zero.  One
+ * launch, a thread per item in a grid-stride loop; nitems == 0 launches nothing. */
+typedef struct {
+  int16_t x, y;  /* block's top-left in the frame, luma px, multiples of 4 (frame_bo.to_luma_plane_offset) */
+  uint8_t bsize; /* BlockSize 0..21 (partition.rs:130-153) */
+  uint8_t skip;  /* the skip choice select_segment is called with */
+  uint8_t pad_[2];
+} b200_segment_item; /* 8 B */
+int b200_select_segment_dev(b200_ctx *ctx, const b200_segment_item *d_items, size_t nitems,
+                            const uint32_t *d_scales, const uint32_t *d_activity, size_t w_imp, size_t h_imp,
+                            int scales_off, int level, const b200_segmentation *d_seg, uint8_t *d_sidx,
+                            uint32_t *d_scale);
+
 /* ---------------------------------------------------------------- quantize chain
  * The steps of encode_tx_block after the forward transform (encoder.rs:1556-1655) for nblocks
  * transform blocks of one (tx_size, tx_type), device-resident:

@@ -125,6 +125,14 @@ assert LOOP_UNIT_DTYPE.itemsize == 28
 ME_RESULT_DTYPE = np.dtype(
     {"names": ["cost", "sad", "mv_row", "mv_col"],
      "formats": ["<u8", "<u4", "<i2", "<i2"], "offsets": [0, 8, 12, 14], "itemsize": 16})
+# b200_segmentation / b200_segment_item (include/b200rdo.h)
+SEGMENTATION_DTYPE = np.dtype([("enabled", "u1"), ("update_data", "u1"), ("update_map", "u1"), ("preskip", "u1"),
+                               ("last_active_segid", "u1"), ("min_segment", "u1"), ("max_segment", "u1"),
+                               ("pad_", "u1"), ("features", "u1", (8, 8)), ("data", "<i2", (8, 8)),
+                               ("threshold", "<u4", (7,)), ("qidx", "u1", (8,)), ("status", "<i4")])
+SEGMENT_ITEM_DTYPE = np.dtype([("x", "<i2"), ("y", "<i2"), ("bsize", "u1"), ("skip", "u1"), ("pad_", "u1", (2,))])
+assert SEGMENTATION_DTYPE.itemsize == 240 and SEGMENT_ITEM_DTYPE.itemsize == 8
+SEGMENTATION_SIMPLE, SEGMENTATION_COMPLEX, SEGMENTATION_FULL = 1, 2, 3  # SegmentationLevel discriminants
 
 BLOCK_SIZES = [(4, 4), (4, 8), (4, 16), (8, 4), (8, 8), (8, 16), (8, 32), (16, 4), (16, 8),
                (16, 16), (16, 32), (16, 64), (32, 8), (32, 16), (32, 32), (32, 64), (64, 16),
@@ -267,6 +275,8 @@ def lib():
     L.b200_block_importances_dev.argtypes = [vp, sz, vp, i32, vp, vp, sz, vp, vp]
     L.b200_distortion_scales_dev.argtypes = [vp, pp, vp, vp, vp]
     L.b200_temporal_scores_dev.argtypes = [vp, sz, sz, vp, vp, vp, vp, vp, sz]
+    L.b200_segmentation_optimize_dev.argtypes = [vp, vp, sz, sz, i32, i32, vp, i32, vp, vp]
+    L.b200_select_segment_dev.argtypes = [vp, vp, sz, vp, vp, sz, sz, i32, i32, vp, vp, vp]
     L.b200_lookahead_motion_dev.argtypes = [vp, sz, vp, vp, C.POINTER(LookaheadMeParams), vp, vp, vp]
     L.b200_get_intra_edges_dev.argtypes = [vp, pp] + [i32] * 7 + [vp, sz, vp, vp]
     L.b200_pred_cfl_ac_dev.argtypes = [vp, pp, vp, sz] + [i32] * 6 + [vp]
@@ -481,6 +491,23 @@ class Context:
         self.check(self.L.b200_temporal_scores_dev(self.h, w_imp, h_imp, _dev_ptr(d_scales), _dev_ptr(d_activity),
                                                    _dev_ptr(d_spatiotemporal), _dev_ptr(d_log_isqrt_mean_scale),
                                                    _dev_ptr(d_scale4x4), scale4x4_stride))
+
+    def segmentation_optimize_dev(self, d_spatiotemporal, w_imp, h_imp, base_q_idx, bit_depth, ac_q, update_data,
+                                  d_prev, d_out):
+        """segmentation_optimize (include/b200rdo.h).  ac_q: the 256-entry ac_qlookup table for bit_depth (host
+        array); d_prev may be None (SegmentationState::default()); d_out receives one SEGMENTATION_DTYPE record."""
+        q = np.ascontiguousarray(ac_q, dtype=np.uint16)
+        assert q.shape == (256,)
+        self.check(self.L.b200_segmentation_optimize_dev(self.h, _dev_ptr(d_spatiotemporal), w_imp, h_imp,
+                                                         int(base_q_idx), int(bit_depth), q.ctypes.data,
+                                                         int(update_data), _dev_ptr(d_prev), _dev_ptr(d_out)))
+
+    def select_segment_dev(self, d_items, n, d_scales, d_activity, w_imp, h_imp, scales_off, level, d_seg, d_sidx,
+                           d_scale=None):
+        """select_segment for n SEGMENT_ITEM_DTYPE items: d_sidx (n x 2 u8) and d_scale (n u32, may be None)."""
+        self.check(self.L.b200_select_segment_dev(self.h, _dev_ptr(d_items), n, _dev_ptr(d_scales),
+                                                  _dev_ptr(d_activity), w_imp, h_imp, int(scales_off), int(level),
+                                                  _dev_ptr(d_seg), _dev_ptr(d_sidx), _dev_ptr(d_scale)))
 
     # ---- RDO cost
     def compute_rd_cost_dev(self, lam, d_rate, d_dist, n, d_cost=None, d_offsets=None, ngroups=0, d_best=None):
