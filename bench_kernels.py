@@ -858,6 +858,57 @@ def segmentation(ctx):
                  cpu=cpu, extra={"items": n, "same_as_oracle": same, "library": lib}, cpu_threads=1)
 
 
+def coeff_rate(ctx):
+    """b200_coeff_rate_dev on two batches, each checked against the oracle, next to the oracle's own rate on all
+    usable host threads:
+    - tx-type decision: every 16x16 block of a seeded 1080p frame quantized by b200_encode_tx_blocks_dev (intra,
+      zero-motion prediction, dc/ac quantizer 140/160) for all 16 types; one chain per (block, type of
+      TX_SET_INTRA_2), the 5 types rdo_tx_type_decision evaluates there, from the default CDFs;
+    - mixed: 4x4 .. 32x32 luma chains of one to four tx blocks plus 4:2:0 chroma chains, seeded coefficients.
+    Symbols: every symbol and bypass bit the chains code (the oracle encoder's count).  Algorithmic bytes per chain:
+    its items, its coded blocks and its output word - what the kernel must read at least.  Downloading the
+    eob-long coefficient runs for the host to count instead moves 2 (i16) bytes per coded position plus the eob:
+    given per line as arithmetic; that alternative's time is not measured."""
+    from tests import coeff_rate_cases as K
+    lib = os.path.basename(B.LIB_PATH)
+    T = K.tx_decision_batch(ctx, 1920, 1080, 8, seed=1)
+    rng = np.random.default_rng(2)
+    b = K.Batch(np.concatenate([K.default_cdfs(), K.random_cdfs(rng, 1)]), 0)
+    for _ in range(6000):
+        t = int(rng.choice([0, 1, 2, 3, 5, 6, 7, 8, 9, 10, 13, 14, 15, 16]))
+        plane = int(rng.choice([0, 0, 1, 2]))
+        w4, h4 = 1 << (K.TX_WL[t] - 2), 1 << (K.TX_HL[t] - 2)
+        items = []
+        for k in range(int(rng.integers(1, 5))):
+            tt = int(rng.choice(K.INV_SET[K.tx_set(t, 0, 0)])) if plane == 0 else 0
+            eob = int(rng.choice(K.eob_choices(rng, t)[:3]))
+            items.append(K.item(b.add_block(K.make_block(rng, t, tt, eob, 0, zero_frac=0.7)), eob, t, tt, plane=plane,
+                                bsize=K.bsize_of(64, 64), x4=(k * w4) % (16 - w4 + 1), y4=0))
+        b.add_chain(items, snapshot=int(rng.integers(0, 5)))
+    batches = [("tx-type decision 1080p 16x16 x 5 intra types", T["cdfs"], T["chains"], T["items"], T["q"]),
+               ("mixed 4x4..32x32 luma + 4:2:0 chroma chains", *b.arrays())]
+    for label, cdfs, chains, items, q in batches:
+        d = [dev(a) for a in (cdfs, chains, items, q)]
+        d_rate = dev(np.zeros(len(chains), np.uint32))
+        d_cul = dev(np.zeros(len(items), np.uint8))
+        call = lambda: ctx.coeff_rate_dev(d[0], len(cdfs), d[1], len(chains), d[2], len(items), d[3], len(q),  # noqa
+                                          int(q.dtype == np.int32), d_rate, d_cul)
+        ms = timed(call, reps=20)
+        want, want_cul = K.oracle_rate(cdfs, chains, items, q)
+        same = bool((d_rate.cpu().numpy().view(np.uint32) == want).all() and (d_cul.cpu().numpy() == want_cul).all())
+        assert same, f"coeff_rate {label} disagrees with the oracle"
+        nsym = sum(K.oracle_encode(cdfs, ch, items, q)[2] for ch in chains[:2000]) * len(chains) / min(2000, len(chains))
+        areas = np.array([K.coded(int(t))[0] * K.coded(int(t))[1] for t in items["tx_size"]])
+        read = (16 * len(items) + q.itemsize * int(areas.sum()) + 112 * len(chains) + 4 * len(chains)) / len(chains)
+        download = (q.itemsize * int(items["eob"].astype(np.int64).sum()) + 2 * len(items)) / len(chains)
+        cpu = cpu_rate(lambda: K.oracle_rate(cdfs, chains, items, q), len(chains))
+        emit(f"coeff_rate_dev {label}", len(chains), "chains", ms, read,
+             "symbols_per_s from the oracle encoder's symbol count (sampled over the first 2000 chains)", cpu=cpu,
+             extra={"items": len(items), "symbols_per_s": nsym / (ms * 1e-3), "same_as_oracle": same,
+                    "host_count_download_bytes_per_chain": download,
+                    "host_count_download_time": "not measured", "library": lib})
+
+
 def main():
     torch.cuda.set_device(0)
     stream = torch.cuda.Stream()
@@ -893,6 +944,9 @@ def main():
         return
     if "--segmentation" in sys.argv[1:]:
         segmentation(ctx)
+        return
+    if "--coeff-rate" in sys.argv[1:]:
+        coeff_rate(ctx)
         return
     rng = np.random.default_rng(0)
     W, H, PAD = 1920, 1080, 96

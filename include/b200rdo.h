@@ -690,6 +690,92 @@ int b200_encode_tx_blocks_dev(b200_ctx *ctx, const b200_plane *cur, const b200_p
                               void *d_coeffs, void *d_qcoeffs, void *d_rcoeffs, uint16_t *d_eob,
                               uint64_t *d_tx_dist);
 
+/* ---------------------------------------------------------------- coefficient rate
+ * The rate term of every transform candidate: what rav1e's WriterCounter reports for the symbols
+ * write_coeffs_lv_map (context/block_unit.rs:1783-2016) codes, counted from a CDF snapshot the caller
+ * provides.  One CHAIN is the ordered list of transform blocks one write_tx_blocks / write_tx_tree call
+ * (or one plane of it) writes through one writer; its items share the writer state (rng), the adapting
+ * CDFs and a window of coefficient contexts.  Per item, in the reference's symbol order:
+ *   txb_skip (get_txb_ctx :442-526) -> eob 0 ends the item with cul_level 0;
+ *   write_tx_type (transform_unit.rs:530-574, luma only) -> encode_eob -> encode_coeffs (reverse scan,
+ *   the base symbol then its br loop) -> encode_coeff_signs (forward: dc_sign, bypass sign bits,
+ *   write_golomb) -> set_coeff_context (:333-348) writes cul_level over the tx block's width_mi /
+ *   height_mi window entries.
+ * Every symbol_with_update adapts the chain's private copy of its snapshot (update_cdf, ec.rs:935-955);
+ * nothing is written back.  d_rate[c] = tell_frac(end) - tell_frac(start) in 1/8 bit (OD_BITRES 3) of a
+ * counter whose rng is chain.init_rng at the start (0x8000 for WriterCounter::new(); a writer that has
+ * already coded mode symbols passes its rng and gets the exact increment, since frac_compute is linear
+ * in the bit count).  It plugs into b200_compute_rd_cost_dev's d_rate unchanged.
+ *
+ * b200_coeff_cdfs holds the coefficient and tx-type fields of CDFContext (context/cdf_context.rs:28-93)
+ * with rav1e's array shapes and element form: u16 inverse CDFs, N slots for N symbols, the adaptation
+ * count in the last slot.  The Rust side copies the fields across unchanged.
+ *
+ * Rules of one call:
+ *  - d_qcoeffs: ncoeffs coefficients, i16 or i32 (coeff_is_i32), holding coded blocks in the layout
+ *    b200_quantize_dev / b200_encode_tx_blocks_dev write.  An item's block starts at coefficient
+ *    item.block * b200_coded_tx_area(item.tx_size): the d_qcoeffs of one such call for the item's size.
+ *    The levels and contexts read the whole coded block (txb_init_levels), not only its first eob.
+ *  - The scan is av1_scan_orders[tx_size][tx_type] (the context's tables, as b200_quantize_dev).
+ *  - Window: above[plane][x4 ..] / left[plane][y4 ..] are the entries get_txb_ctx reads
+ *    (clip_w4 / clip_h4 of them) and set_coeff_context writes (width_mi / height_mi of them).
+ * A chain is INVALID - d_rate[c] = UINT32_MAX, no symbol counted, its items' d_cul_level untouched -
+ * when its snapshot >= ncdfs, init_rng outside 32768..65535, its item range leaves [0, nitems), or any
+ * item has: tx_size >= 19; tx_type >= 16 (WHT_WHT has no scan); plane > 2; plane_bsize >= 22; mode > 33
+ * (NEW_NEWMV), or UV_CFL_PRED (13) on luma; a block reaching past ncoeffs; eob > the coded area; eob > 0 with a zero
+ * coefficient at scan[eob - 1] (get_eob_pos_token would underflow); a coefficient of the coded block equal
+ * to INT16_MIN / INT32_MIN (whose abs() overflows); a luma tx_type its set does not use when eob > 0 and
+ * the set has more than one type (write_tx_type asserts); clip_w4 or clip_h4 of 0; or x4 + max(width_mi,
+ * clip_w4) > 16 or y4 + max(height_mi, clip_h4) > 16.
+ * Rejected with B200_ERR_ARG before any launch, outputs untouched: NULL ctx; nchains > 0 with NULL
+ * d_chains / d_cdfs / d_rate; nitems > 0 with NULL d_items or d_qcoeffs; ncdfs == 0 with nchains > 0;
+ * coeff_is_i32 not 0 / 1; nchains or nitems >= 2^31.  d_cul_level may be NULL: else
+ * d_cul_level[i] is the byte set_coeff_context wrote for item i (0 for eob 0), for the caller to commit
+ * for the candidate it keeps.  Inputs are only read. */
+typedef struct {
+  uint16_t txb_skip[5][13][2];
+  uint16_t dc_sign[2][3][2];
+  uint16_t eob_extra[5][2][9][2];
+  uint16_t eob_flag16[2][2][5];
+  uint16_t eob_flag32[2][2][6];
+  uint16_t eob_flag64[2][2][7];
+  uint16_t eob_flag128[2][2][8];
+  uint16_t eob_flag256[2][2][9];
+  uint16_t eob_flag512[2][2][10];
+  uint16_t eob_flag1024[2][2][11];
+  uint16_t coeff_base_eob[5][2][4][3];
+  uint16_t coeff_base[5][2][42][4];
+  uint16_t coeff_br[5][2][21][4];
+  uint16_t intra_tx_1[4][13][7];
+  uint16_t intra_tx_2[4][13][5];
+  uint16_t inter_tx_1[4][16];
+  uint16_t inter_tx_2[4][12];
+  uint16_t inter_tx_3[4][2];
+} b200_coeff_cdfs; /* 3930 x u16 = 7860 B */
+typedef struct {
+  uint32_t snapshot;   /* index into d_cdfs */
+  uint32_t init_rng;   /* the counter's rng when the chain starts, 32768..65535 */
+  uint32_t item_begin; /* the chain's items are d_items[item_begin .. item_begin + item_count) */
+  uint32_t item_count;
+  uint8_t above[3][16]; /* above_coeff_context window per plane, 4-px units of that plane */
+  uint8_t left[3][16];  /* left_coeff_context window per plane */
+} b200_coeff_chain;     /* 112 B */
+typedef struct {
+  uint32_t block;     /* coded block index in d_qcoeffs */
+  uint16_t eob;       /* 0 ..= coded area */
+  uint8_t tx_size;    /* TxSize 0..18 */
+  uint8_t tx_type;    /* TxType 0..15 */
+  uint8_t plane;      /* 0..2 */
+  uint8_t plane_bsize; /* BlockSize 0..21 of the block in this plane */
+  uint8_t mode;       /* PredictionMode 0..33: inter when >= NEARESTMV (14); the intra direction for luma */
+  uint8_t reduced_tx_set;
+  uint8_t x4, y4;     /* the tx block's first above / left entry in the chain's window */
+  uint8_t clip_w4, clip_h4; /* frame_clipped_txw >> 2, frame_clipped_txh >> 2 (encoder.rs:1561-1566) */
+} b200_coeff_item; /* 16 B */
+int b200_coeff_rate_dev(b200_ctx *ctx, const b200_coeff_cdfs *d_cdfs, size_t ncdfs, const b200_coeff_chain *d_chains,
+                        size_t nchains, const b200_coeff_item *d_items, size_t nitems, const void *d_qcoeffs,
+                        size_t ncoeffs, int coeff_is_i32, uint32_t *d_rate, uint8_t *d_cul_level);
+
 /* Fused residual + transform with resident planes and HOST descriptors / outputs. */
 int b200_fwd_txfm_residual_resident(b200_ctx *ctx, const b200_plane *cur, const b200_plane *ref,
                                     const b200_block *blocks, size_t nblocks,

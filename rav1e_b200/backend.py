@@ -133,6 +133,20 @@ SEGMENTATION_DTYPE = np.dtype([("enabled", "u1"), ("update_data", "u1"), ("updat
 SEGMENT_ITEM_DTYPE = np.dtype([("x", "<i2"), ("y", "<i2"), ("bsize", "u1"), ("skip", "u1"), ("pad_", "u1", (2,))])
 assert SEGMENTATION_DTYPE.itemsize == 240 and SEGMENT_ITEM_DTYPE.itemsize == 8
 SEGMENTATION_SIMPLE, SEGMENTATION_COMPLEX, SEGMENTATION_FULL = 1, 2, 3  # SegmentationLevel discriminants
+# b200_coeff_cdfs / b200_coeff_chain / b200_coeff_item (include/b200rdo.h)
+COEFF_CDFS_DTYPE = np.dtype([("txb_skip", "<u2", (5, 13, 2)), ("dc_sign", "<u2", (2, 3, 2)),
+                             ("eob_extra", "<u2", (5, 2, 9, 2))]
+                            + [(f"eob_flag{16 << i}", "<u2", (2, 2, 5 + i)) for i in range(7)]
+                            + [("coeff_base_eob", "<u2", (5, 2, 4, 3)), ("coeff_base", "<u2", (5, 2, 42, 4)),
+                               ("coeff_br", "<u2", (5, 2, 21, 4)), ("intra_tx_1", "<u2", (4, 13, 7)),
+                               ("intra_tx_2", "<u2", (4, 13, 5)), ("inter_tx_1", "<u2", (4, 16)),
+                               ("inter_tx_2", "<u2", (4, 12)), ("inter_tx_3", "<u2", (4, 2))])
+COEFF_CHAIN_DTYPE = np.dtype([("snapshot", "<u4"), ("init_rng", "<u4"), ("item_begin", "<u4"), ("item_count", "<u4"),
+                              ("above", "u1", (3, 16)), ("left", "u1", (3, 16))])
+COEFF_ITEM_DTYPE = np.dtype([("block", "<u4"), ("eob", "<u2"), ("tx_size", "u1"), ("tx_type", "u1"), ("plane", "u1"),
+                             ("plane_bsize", "u1"), ("mode", "u1"), ("reduced_tx_set", "u1"), ("x4", "u1"),
+                             ("y4", "u1"), ("clip_w4", "u1"), ("clip_h4", "u1")])
+assert COEFF_CDFS_DTYPE.itemsize == 7860 and COEFF_CHAIN_DTYPE.itemsize == 112 and COEFF_ITEM_DTYPE.itemsize == 16
 
 BLOCK_SIZES = [(4, 4), (4, 8), (4, 16), (8, 4), (8, 8), (8, 16), (8, 32), (16, 4), (16, 8),
                (16, 16), (16, 32), (16, 64), (32, 8), (32, 16), (32, 32), (32, 64), (64, 16),
@@ -277,6 +291,7 @@ def lib():
     L.b200_temporal_scores_dev.argtypes = [vp, sz, sz, vp, vp, vp, vp, vp, sz]
     L.b200_segmentation_optimize_dev.argtypes = [vp, vp, sz, sz, i32, i32, vp, i32, vp, vp]
     L.b200_select_segment_dev.argtypes = [vp, vp, sz, vp, vp, sz, sz, i32, i32, vp, vp, vp]
+    L.b200_coeff_rate_dev.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp, sz, i32, vp, vp]
     L.b200_lookahead_motion_dev.argtypes = [vp, sz, vp, vp, C.POINTER(LookaheadMeParams), vp, vp, vp]
     L.b200_get_intra_edges_dev.argtypes = [vp, pp] + [i32] * 7 + [vp, sz, vp, vp]
     L.b200_pred_cfl_ac_dev.argtypes = [vp, pp, vp, sz] + [i32] * 6 + [vp]
@@ -508,6 +523,14 @@ class Context:
         self.check(self.L.b200_select_segment_dev(self.h, _dev_ptr(d_items), n, _dev_ptr(d_scales),
                                                   _dev_ptr(d_activity), w_imp, h_imp, int(scales_off), int(level),
                                                   _dev_ptr(d_seg), _dev_ptr(d_sidx), _dev_ptr(d_scale)))
+
+    def coeff_rate_dev(self, d_cdfs, ncdfs, d_chains, nchains, d_items, nitems, d_qcoeffs, ncoeffs, coeff_is_i32,
+                       d_rate, d_cul_level=None):
+        """write_coeffs_lv_map's rate for nchains COEFF_CHAIN_DTYPE chains (include/b200rdo.h): d_rate (nchains
+        u32, 1/8 bit, UINT32_MAX for an invalid chain) and d_cul_level (nitems u8, may be None)."""
+        self.check(self.L.b200_coeff_rate_dev(self.h, _dev_ptr(d_cdfs), ncdfs, _dev_ptr(d_chains), nchains,
+                                              _dev_ptr(d_items), nitems, _dev_ptr(d_qcoeffs), ncoeffs,
+                                              int(coeff_is_i32), _dev_ptr(d_rate), _dev_ptr(d_cul_level)))
 
     # ---- RDO cost
     def compute_rd_cost_dev(self, lam, d_rate, d_dist, n, d_cost=None, d_offsets=None, ngroups=0, d_best=None):
