@@ -134,13 +134,23 @@ __global__ void __launch_bounds__(256) me_full_search_u8(FsArgs a) {
     {
       const int mis = (int)((uintptr_t)a.ref.data & 3);
       const int ax = ((w.x_lo + mis) & ~3) - mis;  // word-aligned source column
-      const int sh = (w.x_lo - ax) * 8;         // byte realignment
+      const int d = w.x_lo - ax;                   // byte realignment, 0..3
       const uint8_t *src = px<uint8_t>(a.ref, ax, w.y_lo);
+      // Only the row_px bytes [x_lo, x_hi + W) are read: words past them feed only positions beyond
+      // nx and are staged as zeros (the window is clamped to get_mv_range, so those bytes may lie
+      // past the plane's pad).  Each source word loaded holds at least one byte of the row; its
+      // other bytes (up to 3 before x_lo or after x_hi + W - 1, same aligned word) are shifted out.
+      const int need = (row_px + 3) / 4;
       for (int i = threadIdx.x; i < rows * row_words; i += blockDim.x) {
         const int y = i / row_words, k = i - y * row_words;
         const uint32_t *s = (const uint32_t *)(src + (long long)y * a.ref.stride) + k;
-        const uint32_t lo = __ldg(s), hi = __ldg(s + 1);
-        smem[y * pitch_words + k] = __funnelshift_r(lo, hi, sh);
+        uint32_t v = 0u;
+        if (k < need) {
+          const uint32_t lo = __ldg(s);
+          const uint32_t hi = d && 4 * k + 4 - d < row_px ? __ldg(s + 1) : 0u;
+          v = __funnelshift_r(lo, hi, d * 8);
+        }
+        smem[y * pitch_words + k] = v;
       }
     }
     __syncthreads();

@@ -77,6 +77,12 @@ __device__ __forceinline__ uint32_t word_sad(uint32_t a, uint32_t b, uint32_t ac
 // right - needed to realign an unaligned reference row - comes from the neighbouring lane by
 // shuffle; only the last lane of a row segment loads it.  Called by all 32 lanes (candidates that
 // are out of range evaluate the zero vector and are discarded by the caller).
+// Read footprint: with rsh != 0 the aligned-down word of a row starts rsh bytes before the candidate's
+// first column and the extra word ends 4 - rsh bytes past its last, so a candidate on get_mv_range's
+// x_min / x_max touches up to 3 bytes outside min_pad.  Every word loaded still holds a byte of the
+// candidate's row (rsh >= 1 puts the extra word's first byte at or before the row's last byte), so the
+// load stays inside an aligned 4-byte word that is partly readable, and the funnel shift drops the
+// outside bytes: no value outside the footprint reaches a SAD.
 template <typename T>
 __device__ __forceinline__ uint32_t partial_sad(const BlockCtx &c, int dx, int dy, int sub) {
   const uint8_t *r0 = c.ref0 + (long long)(c.po_y + dy) * c.ref_pitch + (long long)(c.po_x + dx) * (long long)sizeof(T);
