@@ -909,6 +909,60 @@ def coeff_rate(ctx):
                     "host_count_download_time": "not measured", "library": lib})
 
 
+def tx_size_type(ctx):
+    """b200_intra_tx_size_type_dev on three 1080p 8-bit luma workloads, each checked against the oracle, next to
+    the oracle (oracle/tx_size_type.c) on all usable host threads:
+    - every 16x16 block x 3 screened modes (DC, V, PAETH), Psychovisual (cdef_dist) distortion;
+    - the same items with tx-domain distortion;
+    - a mixed-size partition: each 32x32 cell split into one of 32x32, 32x16, 16x32, 16x16, 16x8, 8x16, 8x8,
+      one random mode per block.
+    Items carry dc/ac quantizers 120/140 and the default CDFs.  Algorithmic bytes per item: the item, its best
+    record, its 21 candidate records, and the block's src and rec pixels once - what the kernels must touch at
+    least."""
+    from tests import coeff_rate_cases as K
+    from tests import tx_size_type_cases as T
+    lib = os.path.basename(B.LIB_PATH)
+    w, h, pad = 1920, 1080, 64
+    src, rec = T.make_case(w, h, 8, 11)
+    dsrc, drec = ctx.plane_from_host(src, pad), ctx.plane_from_host(rec, pad)
+    cdfs = K.default_cdfs()
+    lam = 0.0013 * 140 * 140
+    rng = np.random.default_rng(12)
+    splits = [(32, 32), (32, 16), (16, 32), (16, 16), (16, 8), (8, 16), (8, 8)]
+    mixed = []
+    for y in range(0, h, 32):
+        for x in range(0, w, 32):
+            bw, bh = splits[int(rng.integers(0, len(splits)))]
+            for yy in range(y, min(y + 32, h), bh):
+                for xx in range(x, x + 32, bw):
+                    mixed.append(T.grid_items(bw, bh, bw, bh, [int(rng.integers(0, 13))]))
+                    mixed[-1]["x"], mixed[-1]["y"] = xx, yy
+    mixed = np.concatenate(mixed)
+    grid = T.grid_items(w, h, 16, 16, [0, 1, 12])
+    loads = [("1080p 16x16 x 3 modes Psychovisual", grid, 2), ("1080p 16x16 x 3 modes tx-domain", grid, 0),
+             ("1080p mixed partition 8x8..32x32 Psychovisual", mixed, 2)]
+    for label, it, dm in loads:
+        n = len(it)
+        d_it, d_cdfs = dev(it), dev(cdfs)
+        d_best = dev(np.zeros(n, B.TX_BEST_DTYPE))
+        d_cands = dev(np.zeros((n, 21), B.TX_CAND_DTYPE))
+        call = lambda: ctx.intra_tx_size_type_dev(drec, dsrc, (0, 0, w, h), w, h, 8, dm, 0, lam, 16384, None, 0,  # noqa
+                                                  d_cdfs, 1, d_it, n, d_best, d_cands)
+        ms = timed(call, reps=10)
+        wb, wc = T.oracle(src, rec, pad, (0, 0, w, h), w, h, 8, dm, 0, lam, 16384, None, cdfs, it)
+        gb = d_best.cpu().numpy().view(B.TX_BEST_DTYPE)
+        gc = d_cands.cpu().numpy().view(B.TX_CAND_DTYPE).reshape(n, 21)
+        same = bool((gb.view(np.uint8) == wb.view(np.uint8)).all() and (gc.view(np.uint8) == wc.view(np.uint8)).all())
+        assert same, f"tx_size_type {label} disagrees with the oracle"
+        px = np.array([T.BS_W[b] * T.BS_H[b] for b in it["bsize"]], np.float64)
+        read = 52 + 16 + 21 * 24 + 2 * float(px.mean())
+        cpu = cpu_rate(lambda: T.oracle(src, rec, pad, (0, 0, w, h), w, h, 8, dm, 0, lam, 16384, None, cdfs, it), n)
+        evaluated = int((gc["state"] == B.TX_EVALUATED).sum())
+        emit(f"intra_tx_size_type_dev {label}", n, "items", ms, read, "items = (block, mode); bytes: item, records, "
+             "src + rec pixels of the block", cpu=cpu,
+             extra={"candidates_evaluated": evaluated, "same_as_oracle": same, "library": lib})
+
+
 def main():
     torch.cuda.set_device(0)
     stream = torch.cuda.Stream()
@@ -947,6 +1001,9 @@ def main():
         return
     if "--coeff-rate" in sys.argv[1:]:
         coeff_rate(ctx)
+        return
+    if "--tx-size-type" in sys.argv[1:]:
+        tx_size_type(ctx)
         return
     rng = np.random.default_rng(0)
     W, H, PAD = 1920, 1080, 96

@@ -776,6 +776,93 @@ int b200_coeff_rate_dev(b200_ctx *ctx, const b200_coeff_cdfs *d_cdfs, size_t ncd
                         size_t nchains, const b200_coeff_item *d_items, size_t nitems, const void *d_qcoeffs,
                         size_t ncoeffs, int coeff_is_i32, uint32_t *d_rate, uint8_t *d_cul_level);
 
+/* ---------------------------------------------------------------- intra transform size and type decision
+ * rdo_tx_size_type (rdo.rs:725-802) for intra luma modes with rdo_tx_decision on (speeds 0-5; that setting
+ * is also tx_mode_select, so the size ladder always runs), with rdo_tx_type_decision (rdo.rs:1701-1823) and
+ * write_tx_blocks' luma loop (encoder.rs:2243-2311 -> encode_tx_block :1404-1658), for a batch of items of
+ * one PlaneRegion (tile).  An item is what luma_chroma_mode_rdo / encode_block call it with: a block, a luma
+ * mode and the quantizers of one segment.  Per item:
+ *  - Size ladder: max_txsize_rect_lookup[bsize], then sub_tx_size_map twice, stopping where the size no
+ *    longer changes.  Per size, the types are RAV1E_TX_TYPES (DCT_DCT, ADST_DCT, DCT_ADST, ADST_ADST, IDTX,
+ *    V_DCT, H_DCT) that av1_tx_used[get_tx_set(size, intra, reduced_tx_set)] keeps; DCT_DCT only for
+ *    TX_SET_DCTONLY or a skip item.  A skip item still codes its coefficients (the reference passes
+ *    skip = false to write_tx_blocks).
+ *  - One candidate (size, type) starts from the item's coefficient-context checkpoint (its above / left
+ *    windows, a private copy of CDF snapshot d_cdfs[snapshot], a WriterCounter at rng 0x8000) and walks the
+ *    size's transform blocks in raster order, skipping a block whose first 4x4 lies at or past the region's
+ *    4x4 extent (ceil(rect_w / 4) x ceil(rect_h / 4)).  Per transform block: get_intra_edges at (bx, by)
+ *    (pixels inside the partition from this candidate's own reconstruction, others from rec),
+ *    predict_intra (angle delta 0, the item's ief, PredictionVariant and the PAETH remap from the transform
+ *    block's tile-relative position), the residual against src (zero when the block is invisible in the
+ *    frame), forward_transform, quantize, write_coeffs_lv_map counted with frame_clipped_txw / txh,
+ *    dequantize, inverse_transform_add when eob > 0 and (the size is not the block's or the distortion is
+ *    pixel-domain), and the tx-domain distortion.
+ *  - Distortion (dist_mode): 0 = tx-domain (Tune::Psnr with tx_domain_distortion): per visible transform
+ *    block its rounded raw distortion times distortion_scale at the block times dist_scale; 1 = sse_wxh
+ *    (Tune::Psnr) and 2 = cdef_dist_wxh (Tune::Psychovisual) over the block's visible area
+ *    (clip_visible_bsize), each chunk times its distortion_scale, the sum times dist_scale.  dist_scale is
+ *    fi.dist_scale[0] (Q14 DistortionScale); d_scale4x4 the per-4x4 luma map b200_weighted_sse_dev takes,
+ *    addressed by frame 4x4 position with scale_stride entries per row; NULL means every distortion_scale is
+ *    the default (temporal RDO off).
+ *  - Cost: rd = compute_rd_cost(lambda, rate, distortion) (f64 fma, as b200_compute_rd_cost_dev).
+ *  - Decision, exactly the reference's: within a size, a first type whose rd > the best rd so far ends the
+ *    size, which then contributes (DCT_DCT, f64::MAX) while the ladder continues; a type replaces the size's
+ *    best only if its rd is strictly less; a size replaces the best only if its rd is strictly less (ties
+ *    keep the larger size).
+ * Every candidate starts from the same checkpoint, so the call evaluates them in parallel and applies the
+ * rules afterwards.  rec is only read: as with b200_cfl_alpha_dev, the caller re-encodes the candidate it
+ * keeps.  What may share a call is the caller's business: each block's neighbours must be final in rec.
+ *
+ * frame_width / frame_height are fi.width / fi.height (clip_visible_bsize, w_in_b / h_in_b).  Outputs:
+ * d_best[i] = the best (tx_size, tx_type) and its rd; d_cands (may be NULL) nitems x 21 records
+ * [item][level * 7 + position in RAV1E_TX_TYPES]: rate (1/8 bit), scaled distortion and rd of every
+ * candidate the reference evaluates, and only the state for the others.
+ * An INVALID item gets {rd -1.0, tx_size 0xFF, tx_type 0xFF} and 21 records of state B200_TX_INVALID, and
+ * nothing is read for it: bsize >= 22 or of the 128 class (13 / 14 / 15), mode >= 13, (x, y) outside the
+ * region or not a multiple of 4, dc_quant or ac_quant outside 1 .. 65535, snapshot >= ncdfs.  (The 16-entry
+ * context windows cover every block up to 64x64, so no window can overflow.)
+ * Rejected with B200_ERR_ARG before any launch, outputs untouched: NULL ctx or planes; a bit depth other
+ * than 8 / 10 / 12 or a bpp that does not match it; rec and src of different sizes; a region outside the
+ * plane or past the frame's 4x4 blocks (4 * w_in_b); a frame larger than the plane; rec->pad or src->pad
+ * below 64 (encode_tx_block's diff reads the whole transform block past the visible frame); dist_mode
+ * outside 0 .. 2; reduced_tx_set not 0 / 1; lambda negative or not finite; a scale map whose stride is below
+ * w_in_b; nitems >= 2^30; with nitems > 0, NULL d_items / d_best / d_cdfs or ncdfs == 0.  nitems == 0
+ * launches nothing.  Context scratch holds the per-size lists (and the records when d_cands is NULL). */
+typedef struct {
+  int16_t x, y;       /* block's top-left inside the region, luma px, multiples of 4 */
+  uint8_t bsize;      /* BlockSize 0..21 without the 128 class */
+  uint8_t mode;       /* luma PredictionMode 0..12 */
+  int8_t ief;         /* -1: enable_intra_edge_filter off; else IntraEdgeFilterParameters::use_smooth_filter() */
+  uint8_t skip;       /* the skip choice the block is evaluated with */
+  uint32_t dc_quant;  /* dc_q / ac_q of get_qidx's qindex, 1..65535 */
+  uint32_t ac_quant;
+  uint32_t snapshot;  /* index into d_cdfs: the CDFs at the block's checkpoint */
+  uint8_t above[16];  /* luma above / left coefficient contexts from the block's first 4x4 */
+  uint8_t left[16];
+} b200_tx_item; /* 52 B */
+typedef struct {
+  double rd;
+  uint8_t tx_size, tx_type; /* TxSize / TxType discriminants */
+  uint8_t pad_[6];
+} b200_tx_best; /* 16 B */
+#define B200_TX_EVALUATED 0
+#define B200_TX_NOT_IN_SET 1    /* av1_tx_used or the DCT-only rule leaves the type out */
+#define B200_TX_CUT 2           /* after the size's first type lost to the best size so far */
+#define B200_TX_NOT_IN_LADDER 3 /* the ladder stopped before this level */
+#define B200_TX_INVALID 255
+typedef struct {
+  double rd;
+  uint64_t dist;  /* ScaledDistortion */
+  uint32_t rate;  /* 1/8 bit */
+  uint32_t state; /* B200_TX_*; rate / dist / rd are 0 unless EVALUATED */
+} b200_tx_cand; /* 24 B */
+int b200_intra_tx_size_type_dev(b200_ctx *ctx, const b200_plane *rec, const b200_plane *src, int rect_x, int rect_y,
+                                int rect_w, int rect_h, int frame_width, int frame_height, int bit_depth,
+                                int dist_mode, int reduced_tx_set, double lambda, uint32_t dist_scale,
+                                const uint32_t *d_scale4x4, size_t scale_stride, const b200_coeff_cdfs *d_cdfs,
+                                size_t ncdfs, const b200_tx_item *d_items, size_t nitems, b200_tx_best *d_best,
+                                b200_tx_cand *d_cands);
+
 /* Fused residual + transform with resident planes and HOST descriptors / outputs. */
 int b200_fwd_txfm_residual_resident(b200_ctx *ctx, const b200_plane *cur, const b200_plane *ref,
                                     const b200_block *blocks, size_t nblocks,

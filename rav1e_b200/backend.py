@@ -147,6 +147,14 @@ COEFF_ITEM_DTYPE = np.dtype([("block", "<u4"), ("eob", "<u2"), ("tx_size", "u1")
                              ("plane_bsize", "u1"), ("mode", "u1"), ("reduced_tx_set", "u1"), ("x4", "u1"),
                              ("y4", "u1"), ("clip_w4", "u1"), ("clip_h4", "u1")])
 assert COEFF_CDFS_DTYPE.itemsize == 7860 and COEFF_CHAIN_DTYPE.itemsize == 112 and COEFF_ITEM_DTYPE.itemsize == 16
+# intra transform size / type decision records (include/b200rdo.h b200_tx_item / b200_tx_best / b200_tx_cand)
+TX_ITEM_DTYPE = np.dtype([("x", "<i2"), ("y", "<i2"), ("bsize", "u1"), ("mode", "u1"), ("ief", "i1"), ("skip", "u1"),
+                          ("dc_quant", "<u4"), ("ac_quant", "<u4"), ("snapshot", "<u4"), ("above", "u1", (16,)),
+                          ("left", "u1", (16,))])
+TX_BEST_DTYPE = np.dtype([("rd", "<f8"), ("tx_size", "u1"), ("tx_type", "u1"), ("pad_", "u1", (6,))])
+TX_CAND_DTYPE = np.dtype([("rd", "<f8"), ("dist", "<u8"), ("rate", "<u4"), ("state", "<u4")])
+TX_EVALUATED, TX_NOT_IN_SET, TX_CUT, TX_NOT_IN_LADDER, TX_INVALID = 0, 1, 2, 3, 255
+assert TX_ITEM_DTYPE.itemsize == 52 and TX_BEST_DTYPE.itemsize == 16 and TX_CAND_DTYPE.itemsize == 24
 
 BLOCK_SIZES = [(4, 4), (4, 8), (4, 16), (8, 4), (8, 8), (8, 16), (8, 32), (16, 4), (16, 8),
                (16, 16), (16, 32), (16, 64), (32, 8), (32, 16), (32, 32), (32, 64), (64, 16),
@@ -292,6 +300,8 @@ def lib():
     L.b200_segmentation_optimize_dev.argtypes = [vp, vp, sz, sz, i32, i32, vp, i32, vp, vp]
     L.b200_select_segment_dev.argtypes = [vp, vp, sz, vp, vp, sz, sz, i32, i32, vp, vp, vp]
     L.b200_coeff_rate_dev.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp, sz, i32, vp, vp]
+    L.b200_intra_tx_size_type_dev.argtypes = [vp, pp, pp] + [i32] * 9 + [C.c_double, C.c_uint32, vp, sz, vp, sz,
+                                                                          vp, sz, vp, vp]
     L.b200_lookahead_motion_dev.argtypes = [vp, sz, vp, vp, C.POINTER(LookaheadMeParams), vp, vp, vp]
     L.b200_get_intra_edges_dev.argtypes = [vp, pp] + [i32] * 7 + [vp, sz, vp, vp]
     L.b200_pred_cfl_ac_dev.argtypes = [vp, pp, vp, sz] + [i32] * 6 + [vp]
@@ -531,6 +541,18 @@ class Context:
         self.check(self.L.b200_coeff_rate_dev(self.h, _dev_ptr(d_cdfs), ncdfs, _dev_ptr(d_chains), nchains,
                                               _dev_ptr(d_items), nitems, _dev_ptr(d_qcoeffs), ncoeffs,
                                               int(coeff_is_i32), _dev_ptr(d_rate), _dev_ptr(d_cul_level)))
+
+    def intra_tx_size_type_dev(self, rec, src, rect, width, height, bit_depth, dist_mode, reduced_tx_set, lam,
+                               dist_scale, d_scale4x4, scale_stride, d_cdfs, ncdfs, d_items, n, d_best, d_cands=None):
+        """rdo_tx_size_type for n TX_ITEM_DTYPE items (include/b200rdo.h): rect = (x, y, w, h) of the tile region;
+        width / height = fi.width / fi.height; dist_mode 0 tx-domain, 1 sse, 2 cdef_dist; d_scale4x4 (per frame
+        4x4, scale_stride entries per row) may be None; d_best (n TX_BEST_DTYPE) and d_cands (n x 21
+        TX_CAND_DTYPE, may be None)."""
+        self.check(self.L.b200_intra_tx_size_type_dev(self.h, C.byref(rec), C.byref(src), rect[0], rect[1], rect[2],
+                                                      rect[3], width, height, bit_depth, dist_mode, reduced_tx_set,
+                                                      float(lam), int(dist_scale), _dev_ptr(d_scale4x4), scale_stride,
+                                                      _dev_ptr(d_cdfs), ncdfs, _dev_ptr(d_items), n, _dev_ptr(d_best),
+                                                      _dev_ptr(d_cands)))
 
     # ---- RDO cost
     def compute_rd_cost_dev(self, lam, d_rate, d_dist, n, d_cost=None, d_offsets=None, ngroups=0, d_best=None):

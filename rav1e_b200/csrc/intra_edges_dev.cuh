@@ -109,11 +109,11 @@ struct EdgeLens {
 };
 
 // Entries rank, rank + nthreads, ... of item e's IntraEdge buffer into out[0..257) (entries outside
-// the initialised slices are zero).  Every thread returns the lengths.
-template <typename T, typename O>
-__device__ EdgeLens gather_intra_edge(const EdgeGeom &a, const b200_edge_item &e, int rank, int nthreads, O *out) {
-  const T *reg = (const T *)a.data;
-  auto PX = [&](int yy, int xx) -> unsigned { return (unsigned)reg[(long long)yy * a.stride + xx]; };
+// the initialised slices are zero), the region's pixels read through PX(y, x) (region coordinates).
+// Every thread returns the lengths.
+template <typename O, typename F>
+__device__ __forceinline__ EdgeLens gather_intra_edge_px(const EdgeGeom &a, const b200_edge_item &e, int rank,
+                                                         int nthreads, O *out, const F &PX) {
   const int x = e.po_x, y = e.po_y;
   const int tx_w = kTxW[e.tx_size], tx_h = kTxH[e.tx_size];
   const unsigned base = 128u << (a.bit_depth - 8);
@@ -191,6 +191,14 @@ __device__ EdgeLens gather_intra_edge(const EdgeGeom &a, const b200_edge_item &e
     out[idx] = (O)v;
   }
   return EdgeLens{init_left, init_above};
+}
+
+// gather_intra_edge_px over the region of a.data.
+template <typename T, typename O>
+__device__ EdgeLens gather_intra_edge(const EdgeGeom &a, const b200_edge_item &e, int rank, int nthreads, O *out) {
+  const T *reg = (const T *)a.data;
+  return gather_intra_edge_px(a, e, rank, nthreads, out,
+                              [&](int yy, int xx) -> unsigned { return (unsigned)reg[(long long)yy * a.stride + xx]; });
 }
 
 }  // namespace intra_edges

@@ -395,10 +395,6 @@ __device__ uint32_t lrf_rate(const Rec &it, int type, int set, int x0, int x1) {
   return bits;
 }
 
-__device__ __forceinline__ double rd_cost(double lambda, uint32_t rate, unsigned long long dist) {
-  return __fma_rn(lambda, (double)rate / 8.0, (double)dist);  // compute_rd_cost, rdo.rs:718-723
-}
-
 __global__ void lrf_search_decide(const __grid_constant__ SearchArgs A) {
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < A.n_items; i += gridDim.x * blockDim.x) {
     b200_lrf_search_item it = A.items[i];

@@ -146,9 +146,13 @@ __global__ void __launch_bounds__(256) quantize_chain_kernel(const __grid_consta
 }
 
 // quantize/mod.rs:129-146
-void divu_gen(uint32_t d, uint32_t out[3]) {
+B200_HD inline void divu_gen(uint32_t d, uint32_t out[3]) {
   const unsigned long long nbits = 32;
+#ifdef __CUDA_ARCH__
+  const unsigned long long m = nbits - (unsigned long long)__clz(d) - 1;
+#else
   const unsigned long long m = nbits - (unsigned long long)__builtin_clz(d) - 1;
+#endif
   if ((d & (d - 1)) == 0) {
     out[0] = out[1] = 0xFFFFFFFFu;
   } else {
@@ -218,15 +222,12 @@ int scan_tables(b200_ctx *ctx, int tx_size, int kind, const uint16_t **d_scan, c
   return B200_OK;
 }
 
-// QuantizationContext::update (quantize/mod.rs:219-267) + the per-call geometry: everything the device
-// code reads except the buffers.
-inline int quant_setup(b200_ctx *ctx, int tx_size, int tx_type, uint32_t dc_quant, uint32_t ac_quant, int is_intra,
-                       int coeff_is_i32, QuantArgs *out) {
-  QuantArgs a{};
-  const int kind = tx_type < 10 ? 0 : ((tx_type & 1) ? 2 : 1);
-  if (int st = scan_tables(ctx, tx_size, kind, &a.scan, &a.iscan)) return st;
-  a.area = kQtxW[tx_size] * kQtxH[tx_size];
-  a.coded = std::min(kQtxW[tx_size], 32) * std::min(kQtxH[tx_size], 32);
+// The step sizes of QuantizationContext::update (quantize/mod.rs:219-267) and the geometry of a w x h
+// transform: on the host (quant_setup) or on the device (per-block quantizers).
+B200_HD inline void quant_params(int w, int h, uint32_t dc_quant, uint32_t ac_quant, int is_intra, int coeff_is_i32,
+                                 QuantArgs &a) {
+  a.area = w * h;
+  a.coded = (w < 32 ? w : 32) * (h < 32 ? h : 32);
   a.log_tx_scale = (a.area > 256) + (a.area > 1024);  // quantize/mod.rs:29-34
   a.dc_quant = dc_quant;
   a.ac_quant = ac_quant;
@@ -239,6 +240,15 @@ inline int quant_setup(b200_ctx *ctx, int tx_size, int tx_type, uint32_t dc_quan
   // deadzone, :287-291: (ac_quant - ac_offset_eob).align_power_of_two_and_shift(log_tx_scale) cast to T
   const size_t dz = ((size_t)ac_quant - ac_offset_eob + ((size_t)1 << a.log_tx_scale) - 1) >> a.log_tx_scale;
   a.deadzone = coeff_is_i32 ? (int)(int32_t)dz : (int)(int16_t)dz;
+}
+
+// quant_params + the scan tables: everything the device code reads except the buffers.
+inline int quant_setup(b200_ctx *ctx, int tx_size, int tx_type, uint32_t dc_quant, uint32_t ac_quant, int is_intra,
+                       int coeff_is_i32, QuantArgs *out) {
+  QuantArgs a{};
+  const int kind = tx_type < 10 ? 0 : ((tx_type & 1) ? 2 : 1);
+  if (int st = scan_tables(ctx, tx_size, kind, &a.scan, &a.iscan)) return st;
+  quant_params(kQtxW[tx_size], kQtxH[tx_size], dc_quant, ac_quant, is_intra, coeff_is_i32, a);
   *out = a;
   return B200_OK;
 }

@@ -15,13 +15,10 @@
 #include <algorithm>
 
 #include "host_stage.cuh"
+#include "rdo_dist_dev.cuh"
 
 namespace {
 
-__device__ __forceinline__ double rd_cost(double lambda, uint32_t rate, unsigned long long dist) {
-  const double rate_in_bits = (double)rate / 8.0;             // rdo.rs:721 (exact)
-  return fma(lambda, rate_in_bits, __ull2double_rn(dist));    // rdo.rs:722
-}
 
 __global__ void rd_cost_kernel(double lambda, const uint32_t *rate, const unsigned long long *dist, size_t n,
                                double *out) {

@@ -3,6 +3,7 @@
 //   get_weighted_sse   src/dist.rs:234-283: one 4x4 chunk's scaled sum, and the final division
 //   cdef_dist_kernel   src/dist.rs:302-372: the five sums -> sse, svar, dvar
 //   apply_ssim_boost   src/activity.rs:159-186 (+ ssim_boost_rsqrt :107-143)
+//   compute_rd_cost    src/rdo.rs:718-723 (see rd_cost.cu)
 #pragma once
 #include "common.cuh"
 
@@ -62,6 +63,11 @@ __device__ __forceinline__ uint32_t cdef_dist_vars(uint32_t sum_s, uint32_t sum_
   *svar_out = (uint32_t)(((unsigned long long)svar * div + (1u << 7)) >> 8);  // scale to an 8x8 area
   *dvar_out = (uint32_t)(((unsigned long long)dvar * div + (1u << 7)) >> 8);
   return sse;
+}
+
+__device__ __forceinline__ double rd_cost(double lambda, uint32_t rate, unsigned long long dist) {
+  const double rate_in_bits = (double)rate / 8.0;             // rdo.rs:721 (exact)
+  return fma(lambda, rate_in_bits, __ull2double_rn(dist));    // rdo.rs:722
 }
 
 }  // namespace
