@@ -718,7 +718,8 @@ int b200_encode_tx_blocks_dev(b200_ctx *ctx, const b200_plane *cur, const b200_p
  *    The levels and contexts read the whole coded block (txb_init_levels), not only its first eob.
  *  - The scan is av1_scan_orders[tx_size][tx_type] (the context's tables, as b200_quantize_dev).
  *  - Window: above[plane][x4 ..] / left[plane][y4 ..] are the entries get_txb_ctx reads
- *    (clip_w4 / clip_h4 of them) and set_coeff_context writes (width_mi / height_mi of them).
+ *    (clip_w4 / clip_h4 of them) and set_coeff_context writes (width_mi / height_mi of them).  An
+ *    entry's sign field (bits 6-7) of 3, which set_coeff_context never writes, counts as no sign.
  * A chain is INVALID - d_rate[c] = UINT32_MAX, no symbol counted, its items' d_cul_level untouched -
  * when its snapshot >= ncdfs, init_rng outside 32768..65535, its item range leaves [0, nitems), or any
  * item has: tx_size >= 19; tx_type >= 16 (WHT_WHT has no scan); plane > 2; plane_bsize >= 22; mode > 33

@@ -314,7 +314,9 @@ typedef struct {
 /* get_txb_ctx, block_unit.rs:442-526 */
 static void get_txb_ctx(const chain_state *cs, const orc_coeff_item *it, int *skip_ctx, int *dc_ctx) {
   const uint8_t *above = &cs->above[it->plane][it->x4], *left = &cs->left[it->plane][it->y4];
-  static const int signs[3] = {0, -1, 1};
+  /* the reference's signs[3] would panic on a sign field of 3, which set_coeff_context never writes; a
+   * caller-built window may hold one, and it counts as no sign (as b200_coeff_rate_dev) */
+  static const int signs[4] = {0, -1, 1, 0};
   int dc_sign = 0;
   for (int i = 0; i < it->clip_w4; i++) dc_sign += signs[above[i] >> 6];
   for (int i = 0; i < it->clip_h4; i++) dc_sign += signs[left[i] >> 6];
