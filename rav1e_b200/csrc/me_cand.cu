@@ -337,11 +337,12 @@ __global__ void __launch_bounds__(SATD ? 128 : B200_SAD_THREADS, (!SATD && W >= 
     // A pass takes `chunk` blocks; it starts as the whole group and halves whenever a window does not
     // fit (e.g. a group that straddles the end of a block row), down to single blocks.
     int chunk = G;
-    bool force_bbox = false;  // set when a hinted window turned out too small for the candidates
+    bool force_bbox = false;  // set when a hinted window does not fit in shared memory
     size_t b0 = gb0, b1 = gb1;
     while (b0 < gb1) {
       const int nb = (int)(b1 - b0);
       __syncthreads();  // previous pass is done with shared memory
+      bool pmv_eq = true;  // this thread's block has p0 == p1
       if (threadIdx.x < nb) {
         const size_t blk = b0 + threadIdx.x;
         const b200_block b = a.blocks[blk];
@@ -351,8 +352,10 @@ __global__ void __launch_bounds__(SATD ? 128 : B200_SAD_THREADS, (!SATD && W >= 
         s_key[threadIdx.x] = ~0ull;
         s_off[threadIdx.x] = a.cand_offsets[blk];
         if (threadIdx.x == nb - 1) s_off[nb] = a.cand_offsets[blk + 1];
+        short pv[4];
 #pragma unroll
-        for (int k = 0; k < 4; k++) s_pmv[threadIdx.x][k] = a.pmv ? a.pmv[4 * blk + k] : (short)0;
+        for (int k = 0; k < 4; k++) s_pmv[threadIdx.x][k] = pv[k] = a.pmv ? a.pmv[4 * blk + k] : (short)0;
+        pmv_eq = pv[0] == pv[2] && pv[1] == pv[3];
       }
       if (threadIdx.x == 32) {
         s_box[0] = INT_MAX;
@@ -360,12 +363,14 @@ __global__ void __launch_bounds__(SATD ? 128 : B200_SAD_THREADS, (!SATD && W >= 
         s_box[2] = INT_MAX;
         s_box[3] = INT_MIN;
       }
-      __syncthreads();
+      // every block of the pass has p0 == p1 (always without a predictor table): the second rate of
+      // b200_mv_cost is then r1 + 1 > r1, and the cooperative path skips it for the whole pass
+      const bool same_pmv = __syncthreads_and(pmv_eq);
       const uint32_t lo = s_off[0], hi = s_off[nb];
       // ---- window extent.  With a search-range hint (cooperative path only) the window is the
       // union of the group's blocks grown by the hint: no pass over the candidates, and staging
-      // can start right away; pass 1 verifies every candidate lies inside and the group falls
-      // back to the exact bounding box below if the hint was wrong.  Otherwise: bounding box of
+      // can start right away; pass 1 checks every candidate against it, and a candidate the hint
+      // does not cover is evaluated by its own lane from the reference plane.  Otherwise: bounding box of
       // the in-range candidates (reference coordinates of the block top-left).
       const bool hinted = COOP && a.hint_px > 0 && !force_bbox;
       // hinted: the first round's candidate is fetched now, under the window staging
@@ -462,7 +467,7 @@ __global__ void __launch_bounds__(SATD ? 128 : B200_SAD_THREADS, (!SATD && W >= 
           continue;
         }
       }
-      if (!fits && hinted) {  // the exact bounding box may still fit
+      if (!fits && hinted) {  // a hint wider than shared memory: the exact bounding box may still fit
         force_bbox = true;
         continue;
       }
@@ -494,57 +499,54 @@ __global__ void __launch_bounds__(SATD ? 128 : B200_SAD_THREADS, (!SATD && W >= 
       __syncthreads();
 
       if (COOP && staged) {
-        // Pass 1 (thread per candidate): range check and addresses -> one uint4 per candidate:
-        //   {shared address of the candidate's first footprint word, shared address of its
-        //    block's org words, funnel shift, 0}.  Out-of-range candidates point at the window
-        //   origin: they are evaluated like the others (no divergence) and discarded afterwards.
-        // Pass 2 (warp per 32 candidates, fully unrolled): one broadcast LDS.128 fetches the
+        // Pass 1 (thread per candidate): range check and addresses -> one 8-byte record per candidate:
+        //   {shared address of the candidate's first footprint word, shared address of its block's org
+        //    words << 3 | funnel shift}.  The funnel shift reads the low 5 bits of the second word, and an
+        //   org address is a multiple of 4, so the shift needs no word of its own.  Out-of-range
+        //   candidates, and in-range ones the hinted window does not cover, point at the window origin:
+        //   the loop evaluates them like the others (no divergence) and the result is discarded.
+        // Pass 2 (warp per 32 candidates, fully unrolled): one broadcast LDS.64 fetches the
         //   parameters, each lane loads its (row, word) of the footprint and of org with plain
-        //   32-bit shared addresses, REDUX.SUM hands the SAD to the owner lane.
-        __shared__ uint4 s_par[nthr];
+        //   32-bit shared addresses, REDUX.SUM hands the SAD to the owner lane.  s_par is per warp,
+        //   so a round needs no CTA barrier.
+        // A candidate outside the hinted window takes its SAD from the reference plane in its own
+        // lane after the loop.
+        __shared__ uint2 s_par[nthr];
         const int warp = threadIdx.x >> 5;
         const int lrow = lane / LPR, lword = lane - lrow * LPR;
         const uint32_t win_s = smem_u32(win), org_s = smem_u32(s_org);
         const uint32_t lane_win = (uint32_t)(lrow * pitch_words + lword) * 4u;
         const uint32_t lane_org = (uint32_t)(lrow * (W / 4) + lword) * 4u;
         const uint32_t pstep = (uint32_t)(RPP * pitch_words) * 4u;
-        bool hint_failed = false;
         for (uint32_t base = lo; base < hi; base += nthr) {
           const uint32_t i = base + threadIdx.x;
           const bool valid = i < hi;
-          bool inr = false;
-          int outside = 0;
+          bool inr = false, outside = false;
           b200_cand cd;
           cd.block = 0;
           cd.mv_row = 0;
           cd.mv_col = 0;
           int lb = 0;
-          uint4 par = make_uint4(win_s, org_s, 0u, 0u);
+          uint2 par = make_uint2(win_s, org_s << 3);
           if (valid) {
             cd = (hinted && base == lo) ? pre : a.cands[i];
             lb = (int)(cd.block - (uint32_t)b0);
             const MvRange r = s_rng[lb];
             inr = !B200_MV_OUTSIDE(cd.mv_row, cd.mv_col, r);
             if (inr) {
-              const int off = s_blk[lb].x + cd.mv_col / 8 - wx0;
-              const int roff = s_blk[lb].y + cd.mv_row / 8 - wy0;
+              const b200_block b = s_blk[lb];
+              const int off = b.x + cd.mv_col / 8 - wx0;
+              const int roff = b.y + cd.mv_row / 8 - wy0;
               outside = off < 0 || off + W + 4 > row_bytes || roff < 0 || roff + H > rows;
-              par.x = win_s + (uint32_t)(roff * pitch_words + (off >> 2)) * 4u;
-              par.y = org_s + (uint32_t)(lb * ORGW) * 4u;
-              par.z = (uint32_t)(off & 3) * 8u;
+              if (!outside) {
+                par.x = win_s + (uint32_t)(roff * pitch_words + (off >> 2)) * 4u;
+                par.y = ((org_s + (uint32_t)(lb * ORGW) * 4u) << 3) | (uint32_t)(off & 3) * 8u;
+              }
             }
           }
-          // (also retires the previous round's readers of s_par)
-          if (hinted ? __syncthreads_or(outside) : (__syncthreads(), 0)) {
-            hint_failed = true;  // uniform
-            if (by_tma && base == lo) {  // the copy in flight must land before the window is reused
-              mbar_wait(mbar, tma_parity);
-              tma_parity ^= 1;
-            }
-            break;
-          }
+          __syncwarp();  // the warp's previous round has read its s_par slots
           s_par[threadIdx.x] = par;
-          __syncthreads();
+          __syncwarp();
           if (by_tma && base == lo) {  // window bytes arrive here, behind pass 1
             mbar_wait(mbar, tma_parity);
             tma_parity ^= 1;
@@ -552,14 +554,16 @@ __global__ void __launch_bounds__(SATD ? 128 : B200_SAD_THREADS, (!SATD && W >= 
           uint32_t sad = 0;
           const uint32_t par_s = smem_u32(s_par + warp * 32);
           // When the warp's 32 candidates belong to one block (the usual case: lists are grouped
-          // by block) its org words are loaded into registers once instead of per candidate.
+          // by block) its org words are loaded into registers once instead of per candidate, and
+          // its first minimum is one 32-bit REDUX.
           // (out-of-range / padding lanes are ignored: their result is discarded anyway)
           const unsigned live = __ballot_sync(0xffffffffu, inr);
-          const uint32_t org0 = __shfl_sync(0xffffffffu, par.y, live ? __ffs(live) - 1 : 0);
-          const bool one_block = __all_sync(0xffffffffu, !inr || par.y == org0);
+          const int lb0 = __shfl_sync(0xffffffffu, lb, live ? __ffs(live) - 1 : 0);
+          const bool one_block = __all_sync(0xffffffffu, !inr || lb == lb0);
           if (!live) {
             // nothing in range in this warp's 32 slots (the tail of a group's last round): skip the evaluation
           } else if (one_block) {
+            const uint32_t org0 = org_s + (uint32_t)(lb0 * ORGW) * 4u;
             uint32_t orgr[P];
 #pragma unroll
             for (int p = 0; p < P; p++)
@@ -568,10 +572,8 @@ __global__ void __launch_bounds__(SATD ? 128 : B200_SAD_THREADS, (!SATD && W >= 
                            : "r"(org0 + lane_org + (uint32_t)(p * RPP * (W / 4)) * 4u));
 #pragma unroll
             for (int sidx = 0; sidx < 32; sidx++) {
-              uint32_t qa, qo, qs, qz;
-              asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];"
-                           : "=r"(qa), "=r"(qo), "=r"(qs), "=r"(qz)
-                           : "r"(par_s + (uint32_t)sidx * 16u));
+              uint32_t qa, qs;
+              asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(qa), "=r"(qs) : "r"(par_s + (uint32_t)sidx * 8u));
               uint32_t wa = qa + lane_win;
               uint32_t part = 0;
 #pragma unroll
@@ -588,12 +590,10 @@ __global__ void __launch_bounds__(SATD ? 128 : B200_SAD_THREADS, (!SATD && W >= 
           } else {
 #pragma unroll
             for (int sidx = 0; sidx < 32; sidx++) {
-              uint32_t qa, qo, qs, qz;
-              asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];"
-                           : "=r"(qa), "=r"(qo), "=r"(qs), "=r"(qz)
-                           : "r"(par_s + (uint32_t)sidx * 16u));
+              uint32_t qa, qs;
+              asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(qa), "=r"(qs) : "r"(par_s + (uint32_t)sidx * 8u));
               uint32_t wa = qa + lane_win;
-              const uint32_t oa = qo + lane_org;
+              const uint32_t oa = ((qs >> 3) & ~3u) + lane_org;  // drop the shift's (off & 3)
               uint32_t part = 0;
 #pragma unroll
               for (int p = 0; p < P; p++) {
@@ -608,11 +608,24 @@ __global__ void __launch_bounds__(SATD ? 128 : B200_SAD_THREADS, (!SATD && W >= 
               keep_if_lane(sad, tot, lane, sidx);
             }
           }
-          unsigned long long cost = kEmptyCost, key = ~0ull;
+          if (outside) {  // in range, beyond the hinted window: the non-staged form, from the plane
+            const b200_block b = s_blk[lb];
+            const uint8_t *rp = px<uint8_t>(ref, b.x + cd.mv_col / 8, b.y + cd.mv_row / 8);
+            const int gsh = (int)((uintptr_t)rp & 3);
+            const uint32_t *gw = (const uint32_t *)(rp - gsh);
+            const uint32_t *org = s_org + lb * ORGW;
+            sad = 0;
+            for (int y = 0; y < H; y++)
+              sad = row_sad_u8<W>(gw + (long long)y * (ref.stride >> 2), 0, gsh * 8, org + y * (W / 4), sad);
+          }
+          unsigned long long cost = kEmptyCost;
           if (inr) {
-            cost = b200_mv_cost(sad, cd.mv_row, cd.mv_col, s_pmv[lb][0], s_pmv[lb][1], s_pmv[lb][2],
-                                s_pmv[lb][3], a.lambda, a.allow_hp);
-            key = pack_key(cost, i - s_off[lb]);
+            uint32_t rate = b200_mv_rate(cd.mv_row, cd.mv_col, s_pmv[lb][0], s_pmv[lb][1], a.allow_hp);
+            if (!same_pmv) {
+              const uint32_t r2 = b200_mv_rate(cd.mv_row, cd.mv_col, s_pmv[lb][2], s_pmv[lb][3], a.allow_hp) + 1;
+              rate = r2 < rate ? r2 : rate;
+            }
+            cost = 256ull * sad + (unsigned long long)rate * a.lambda;  // b200_mv_cost
           } else {
             sad = kEmptySad;
             lb = -1;
@@ -621,11 +634,17 @@ __global__ void __launch_bounds__(SATD ? 128 : B200_SAD_THREADS, (!SATD && W >= 
             if (a.out_sad) a.out_sad[i] = sad;
             if (a.out_cost) a.out_cost[i] = cost;
           }
-          if (a.out_best) warp_keys_into(s_key, key, lb, lane);
-        }
-        if (hint_failed) {  // redo this pass with the exact bounding box (results are rewritten)
-          force_bbox = true;
-          continue;
+          if (a.out_best) {
+            if (one_block && a.key32) {
+              // (cost, lane) in 32 bits orders like (cost, index) inside the warp; the winning lane
+              // folds its 64-bit key into the block's minimum
+              const uint32_t k = inr ? ((uint32_t)cost << 5) | (uint32_t)lane : ~0u;
+              const uint32_t kmin = __reduce_min_sync(0xffffffffu, k);
+              if (k == kmin && inr) atomicMin(&s_key[lb], pack_key(cost, i - s_off[lb]));
+            } else {
+              warp_keys_into(s_key, inr ? pack_key(cost, i - s_off[lb]) : ~0ull, lb, lane);
+            }
+          }
         }
       } else {
       // ---- evaluate: each slot of TPC threads takes candidates lo+slot, lo+slot+nslots, ...
@@ -1053,6 +1072,10 @@ int launch_cand_group(b200_ctx *ctx, MeArgs a, int window_hint_px, const b200_pl
   }
   smem = std::min<size_t>(std::max<size_t>(smem, 16 * 1024), (size_t)kCandSmemBytes);
   a.smem_bytes = (int)smem;
+  // 32-bit warp keys when the largest possible cost, 256 * 255 * W * H + 64 * lambda (a rate is two
+  // b200_diff_to_rate terms of at most 2 * 16), leaves (cost << 5 | 31) below ~0u; the 64-bit key is
+  // the only exact form above that
+  a.key32 = 256ull * 255 * W * H + 64ull * a.lambda < (1ull << 27) - 1;
   // groups never straddle a plane pair
   size_t ngroups = 0;
   uint32_t b0 = a.pr.block_begin;

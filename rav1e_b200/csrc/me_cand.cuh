@@ -38,6 +38,9 @@ struct MeArgs {
   int smem_bytes;  // dynamic smem given to the staged kernels
   size_t ngroups;  // ceil(nblocks / G) for the grouped kernel
   int hint_px;     // caller's bound on |mv|/8 (0 = unknown)
+  // cooperative SAD kernel: every cost of the launch is below 2^27 - 1, so (cost << 5 | lane) is an
+  // exact 32-bit warp key (launch_cand_group, from w, h, lambda and the largest rate)
+  int key32;
   MePairs pr;
 };
 
