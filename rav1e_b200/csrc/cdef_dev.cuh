@@ -1,7 +1,7 @@
 // cdef_dev.cuh — the CDEF device primitives (rav1e src/cdef.rs): direction search of one 8x8 block,
 // the constrain / adjust_strength helpers, the per-block strength and direction set-up of
 // cdef_filter_superblock and the per-pixel filter over an int16 tile that carries the sentinel.
-// Used by the frame-level kernels (cdef.cu) and the fused loop-filter RDO (cdef_rdo.cu).
+// Used by the frame-level kernels (cdef.cu) and the loop-filter RDO superblock (cdef_sb_dev.cuh).
 #pragma once
 #include "common.cuh"
 

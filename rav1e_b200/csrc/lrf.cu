@@ -21,6 +21,7 @@
 
 #include "common.cuh"
 #include "host_stage.cuh"
+#include "loop_filter_checks.cuh"
 #include "lrf_dev.cuh"
 
 namespace {
@@ -214,8 +215,6 @@ __global__ void __launch_bounds__(kThreads) lrf_filter_kernel(const LrfArgs a) {
   }
 }
 
-bool is_pow2_unit(int s) { return s >= 32 && s <= 256 && (s & (s - 1)) == 0; }
-
 // bytes [lo, hi) a plane's crop rect spans
 struct Span {
   uintptr_t lo, hi;
@@ -231,8 +230,8 @@ int check_unit(b200_ctx *ctx, const b200_lrf_unit &r, int p, size_t i) {
   B200_REQUIRE(ctx, r.type <= 2, "plane %d unit %zu: type %d", p, i, r.type);
   if (r.type == 2) {
     B200_REQUIRE(ctx, r.set <= 15, "plane %d unit %zu: sgrproj set %d", p, i, r.set);
-    B200_REQUIRE(ctx, r.xqd[0] >= -96 && r.xqd[0] <= 31 && r.xqd[1] >= -32 && r.xqd[1] <= 95,
-                 "plane %d unit %zu: xqd (%d, %d) out of range", p, i, r.xqd[0], r.xqd[1]);
+    B200_REQUIRE(ctx, sgrproj_xqd_ok(r.xqd[0], r.xqd[1]), "plane %d unit %zu: xqd (%d, %d) out of range", p, i,
+                 r.xqd[0], r.xqd[1]);
   } else if (r.type == 1) {
     for (int d = 0; d < 2; d++)
       for (int k = 0; k < 3; k++)
@@ -267,7 +266,7 @@ extern "C" int b200_lrf_filter_dev(b200_ctx *ctx, const b200_plane *cdeffed, con
     const long long cw = ((long long)frame_width + (1 << xd >> 1)) >> xd;
     const long long ch = ((long long)frame_height + (1 << yd >> 1)) >> yd;
     cwv[p] = cw, chv[p] = ch;
-    B200_REQUIRE(ctx, is_pow2_unit(unit_size[p]), "plane %d: unit size %d is not a power of two in 32..256", p,
+    B200_REQUIRE(ctx, lrf_unit_size_ok(unit_size[p]), "plane %d: unit size %d is not a power of two in 32..256", p,
                  unit_size[p]);
     B200_REQUIRE(ctx, units[p] != nullptr, "NULL units for plane %d", p);
     for (const b200_plane *pl : {cdeffed, deblocked, out}) {

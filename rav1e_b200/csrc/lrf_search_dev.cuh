@@ -1,12 +1,13 @@
-// lrf_search_dev.cuh — the restoration search's kernels (rav1e src/rdo.rs:2575-2740), shared by the search
-// entry point (lrf_search.cu) and the pass loop of rdo_loop_decision (loop_decision.cu), which launches them
-// once per restoration stage with the incumbents carried on the device.  The self-guided tile pieces
-// (staging through setup_integral_image's clip rule, box sums, a / b, the two filter outputs) are also the
-// C stage's Sgrproj branch.  See lrf_search.cu for the launch sequence.
+// lrf_search_dev.cuh — what the restoration search (rav1e src/rdo.rs:2575-2740) shares between its two
+// callers, b200_lrf_search_dev and the L stage of b200_loop_decision_dev's pass loop: the argument types and
+// lrf_search_launch (its kernels and launch sequence are in lrf_search.cu), the per-item host set-up, and the
+// pieces the pass loop's C stage also runs for its Sgrproj branch: the self-guided tile steps (staging through
+// setup_integral_image's clip rule, box sums, a / b, the two filter outputs) and lrf_rate.
 #pragma once
 #include <algorithm>
 #include <vector>
 
+#include "host_stage.cuh"
 #include "lrf_dev.cuh"
 #include "rdo_dist_dev.cuh"
 
@@ -18,6 +19,11 @@ constexpr int kSP = kT + 6;         // staged pixels per side: the tile plus 3 o
 constexpr int kAB = kT + 2;         // a / b columns (and radius-1 rows): -1 .. kT
 constexpr int kR2 = kT / 2 + 1;     // radius-2 a / b rows: the odd rows -1 .. kT - 1
 constexpr int kCands = 17;          // None, then sets 0 .. 15
+
+}  // namespace
+
+// named, because lrf_search_launch is called from two translation units
+namespace lrf_search {
 
 struct Tile {
   uint32_t item;
@@ -60,6 +66,19 @@ struct SearchArgs {
   const uint8_t *active;    // [area] areas still in the pass loop; the others' items are skipped
   uint8_t *area_changed;    // [area] set when a unit of the area changes
 };
+
+// Zeroes a.acc / a.err (n_items x 16 x 5 and n_items x kCands) and makes the search's four launches on the
+// context's stream: the tile statistics, the solve, the tile errors and the decision.  On a failed memset it
+// returns s.finish(false).
+int lrf_search_launch(b200_ctx *ctx, HostStage &s, const SearchArgs &a);
+
+}  // namespace lrf_search
+
+namespace {
+
+using lrf_search::Geo;
+using lrf_search::SearchArgs;
+using lrf_search::Tile;
 
 // setup_integral_image's clip rule (lrf.rs:529-627) for a unit at (po_x, po_y) of its area with visible rect
 // vis_w x vis_h: columns clamp to [0, po_x + vis_w) of the area (4 real columns on the left, none past the
@@ -155,12 +174,33 @@ __device__ __forceinline__ uint16_t sgr_apply(int w0, int w1, int w2, uint32_t f
   return (uint16_t)min(max((v + (1 << 10)) >> 11, 0), (1 << bd) - 1);
 }
 
-// a unit's geometry in its plane's pixels (rdo.rs:2651-2658; the area's scratch rect, rdo.rs:2152-2157);
-// the unit is inside its area when lru_x * lru_sb_w < sb_w and likewise vertically
-inline Geo lrf_unit_geo(const b200_cdef_rdo_area &r, int p, int xd, int yd, int us, int lru_x, int lru_y,
-                        int frame_width, int frame_height) {
-  Geo g;
+// the SearchArgs fields both callers fill alike; `in` is the plane list the units are filtered from
+inline SearchArgs search_args(const b200_plane *in, const b200_plane *src, int planes, int xdec, int ydec,
+                              int bit_depth, int frame_width, int reduced_sets, const uint32_t *d_imp_scales,
+                              const uint32_t dist_scale[3], double lambda) {
+  SearchArgs a{};
+  for (int p = 0; p < planes; p++) {
+    a.in[p] = PlaneView{in[p].data, in[p].stride};
+    a.src[p] = PlaneView{src[p].data, src[p].stride};
+    a.dist_scale[p] = dist_scale[p];
+  }
+  a.xdec = xdec, a.ydec = ydec, a.bit_depth = bit_depth, a.w8 = (frame_width + 7) >> 3;
+  a.reduced = reduced_sets != 0;
+  a.nsets = a.reduced ? 8 : 16;
+  a.imp = d_imp_scales;
+  a.lambda = lambda;
+  return a;
+}
+
+// Unit (lru_x, lru_y) of plane p in area r, item or unit `i` of the call: its geometry in the plane's pixels
+// (rdo.rs:2651-2658; the area's scratch rect, rdo.rs:2152-2157).  Rejects a unit outside its area or the
+// visible frame.
+inline int lrf_item_geo(b200_ctx *ctx, size_t i, const b200_cdef_rdo_area &r, int p, int xdec, int ydec, int us,
+                        int lru_x, int lru_y, int frame_width, int frame_height, Geo &g) {
+  const int xd = p ? xdec : 0, yd = p ? ydec : 0;
   const int lsw = (us << xd) / 64, lsh = (us << yd) / 64;
+  B200_REQUIRE(ctx, lru_x >= 0 && lru_y >= 0 && lru_x * lsw < r.sb_w && lru_y * lsh < r.sb_h,
+               "unit %zu: (%d, %d) outside its %dx%d area", i, lru_x, lru_y, r.sb_w, r.sb_h);
   g.ax = (r.sbx * 64) >> xd, g.ay = (r.sby * 64) >> yd;
   const int crop_w = frame_width - r.sbx * 64, crop_h = frame_height - r.sby * 64;
   g.po_x = (lru_x * lsw * 64) >> xd, g.po_y = (lru_y * lsh * 64) >> yd;
@@ -169,196 +209,14 @@ inline Geo lrf_unit_geo(const b200_cdef_rdo_area &r, int p, int xd, int yd, int 
   g.ew = std::min(us, (aw >> xd) - g.po_x), g.eh = std::min(us, (ah >> yd) - g.po_y);
   g.gbx0 = r.sbx * 8 + lru_x * lsw * 8, g.gby0 = r.sby * 8 + lru_y * lsh * 8;
   g.p = p, g.xd = xd, g.yd = yd;
-  return g;
+  B200_REQUIRE(ctx, g.vis_w > 0 && g.vis_h > 0, "unit %zu: (%d, %d) outside the visible frame", i, lru_x, lru_y);
+  return B200_OK;
 }
 
-__device__ __forceinline__ int set_of(const SearchArgs &A, int si) { return A.reduced ? 2 * si + 1 : si; }
-
-template <typename T, bool ERR>
-__global__ void __launch_bounds__(kThreads) lrf_search_tiles(const __grid_constant__ SearchArgs A) {
-  __shared__ uint16_t sp[kSP][kSP];            // lrf_in through the clip rule
-  __shared__ uint16_t ss[kT][kT];              // src
-  __shared__ uint16_t st[kT][kT];              // ERR: the candidate's test pixels
-  __shared__ uint32_t box1[2][kAB][kAB];       // radius-1 sum / sum of squares
-  __shared__ uint32_t box2[2][kR2][kAB];       // radius-2 sum / sum of squares
-  __shared__ uint32_t a1[kAB][kAB], b1[kAB][kAB], a2[kR2][kAB], b2[kR2][kAB];
-  __shared__ unsigned long long red[kThreads / 32][5];
-
-  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
-  const int bd = A.bit_depth, bdm8 = bd - 8;
-  for (uint32_t k = blockIdx.x; k < A.n_tiles; k += gridDim.x) {
-    const Tile tl = A.tiles[k];
-    if (A.active && !A.active[A.items[tl.item].area]) continue;
-    const Geo g = A.geo[tl.item];
-    const int tx = tl.tx, ty = tl.ty;
-    const T *in = (const T *)A.in[g.p].data + (long long)g.ay * A.in[g.p].stride + g.ax;
-    const T *sr = (const T *)A.src[g.p].data + (long long)g.ay * A.src[g.p].stride + g.ax;
-    const int is = A.in[g.p].stride, ssd = A.src[g.p].stride;
-    sgr_stage_tile<T>(sp, in, is, g.po_x, g.po_y, g.vis_w, g.vis_h, tx, ty);
-    const int tw = min(kT, g.ew - tx), th = min(kT, g.eh - ty);  // the tile's part of the unit's blocks
-    for (int i = t; i < kT * kT; i += kThreads) {
-      const int r = i / kT, c = i - r * kT;
-      ss[r][c] = r < th && c < tw ? (uint16_t)sr[(long long)(g.po_y + ty + r) * ssd + g.po_x + tx + c] : 0;
-    }
-    __syncthreads();
-    sgr_box_sums(sp, box1, box2);
-
-    // ERR: the unit's 8x8 blocks in this tile, one thread each (rdo_loop_plane_error)
-    const int bw = 8 >> g.xd, bh = 8 >> g.yd, nbx = kT / bw, nb = nbx * (kT / bh);
-    const int bx = t % nbx, by = t / nbx;
-    const bool blk = ERR && t < nb && bx * bw < tw && by * bh < th;
-    uint32_t bias = 1u << 14;
-    if (blk && A.imp) bias = A.imp[(size_t)(g.gby0 + ((ty + by * bh) / bh)) * A.w8 + g.gbx0 + (tx + bx * bw) / bw];
-    auto block_err = [&]() -> unsigned long long {  // of st against ss
-      if (!blk) return 0ull;
-      const int x0 = bx * bw, y0 = by * bh;
-      if (g.p == 0) {  // cdef_dist_kernel 8x8 times the bias (mul_u64)
-        uint32_t s1 = 0, d1 = 0, s2 = 0, d2 = 0, sd = 0;
-        for (int r = 0; r < 8; r++)
-          for (int c = 0; c < 8; c++) {
-            const uint32_t s = ss[y0 + r][x0 + c], d = st[y0 + r][x0 + c];
-            s1 += s, d1 += d, s2 += s * s, d2 += d * d, sd += s * d;
-          }
-        uint32_t sv, dv;
-        const uint32_t sse = cdef_dist_vars(s1, d1, s2, d2, sd, 64, &sv, &dv);
-        return ((unsigned long long)bias * apply_ssim_boost(sse, sv, dv, bd) + (1u << 13)) >> 14;
-      }
-      unsigned long long acc = 0;  // sse_wxh: get_weighted_sse with the bias on every 4x4 chunk
-      for (int cy = 0; cy < bh; cy += 4)
-        for (int cx = 0; cx < bw; cx += 4) {
-          uint32_t e = 0;
-          for (int r = 0; r < 4; r++)
-            for (int c = 0; c < 4; c++) {
-              const int d = (int)ss[y0 + cy + r][x0 + cx + c] - (int)st[y0 + cy + r][x0 + cx + c];
-              e += (uint32_t)(d * d);
-            }
-          acc += wsse_chunk(e, bias);
-        }
-      return wsse_finish(acc);
-    };
-    auto reduce_add = [&](unsigned long long v, unsigned long long *dst) {
-#pragma unroll
-      for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-      if (lane == 0) red[warp][0] = v;
-      __syncthreads();
-      if (t == 0) {
-        unsigned long long s = 0;
-        for (int w = 0; w < kThreads / 32; w++) s += red[w][0];
-        atomicAdd(dst, s);
-      }
-    };
-    if (ERR) {  // the None candidate: lrf_in itself over the blocks
-      for (int i = t; i < kT * kT; i += kThreads) {
-        const int r = i / kT, c = i - r * kT;
-        st[r][c] = r < th && c < tw ? (uint16_t)in[(long long)(g.po_y + ty + r) * is + g.po_x + tx + c] : 0;
-      }
-      __syncthreads();
-      reduce_add(block_err(), &A.err[(size_t)tl.item * kCands]);
-    }
-
-    for (int si = 0; si < A.nsets; si++) {
-      const int set = set_of(A, si);
-      const uint32_t s2 = kSgrS[set][0], s1 = kSgrS[set][1];
-      __syncthreads();
-      sgr_ab(box1, box2, a1, b1, a2, b2, s1, s2, bdm8);
-      __syncthreads();
-      int w0 = 0, w1 = 0, w2 = 0;
-      if (ERR) {
-        const int8_t *q = &A.xq[((size_t)tl.item * 16 + set) * 2];
-        w0 = q[0], w1 = q[1], w2 = 128 - w0 - w1;
-      }
-      long long h00 = 0, h11 = 0, h01 = 0, c0 = 0, c1 = 0;
-      for (int i = t; i < kT * kT; i += kThreads) {
-        const int y = i / kT, x = i - y * kT;
-        const bool vis = tx + x < g.vis_w && ty + y < g.vis_h;
-        if (!vis) {
-          if (ERR) st[y][x] = B200_LRF_WORK_FILL;
-          continue;
-        }
-        uint32_t f1, f2;
-        const uint32_t px = sgr_f(sp, a1, b1, a2, b2, s1, s2, y, x, f1, f2);
-        const int u = (int)(px << 4);
-        if (ERR) {
-          st[y][x] = sgr_apply(w0, w1, w2, f1, f2, px, bd);
-        } else {  // process_line (lrf.rs:997-1037)
-          const long long s = (long long)(((int)ss[y][x] << 4) - u), e2 = (int)f2 - u, e1 = (int)f1 - u;
-          h00 += e2 * e2;
-          h11 += e1 * e1;
-          h01 += e1 * e2;
-          c0 += e2 * s;
-          c1 += e1 * s;
-        }
-      }
-      if (ERR) {
-        __syncthreads();
-        reduce_add(block_err(), &A.err[(size_t)tl.item * kCands + 1 + set]);
-      } else {
-        long long v[5] = {h00, h11, h01, c0, c1};
-#pragma unroll
-        for (int q = 0; q < 5; q++) {
-#pragma unroll
-          for (int o = 16; o; o >>= 1) v[q] += __shfl_xor_sync(0xffffffffu, v[q], o);
-          if (lane == 0) red[warp][q] = (unsigned long long)v[q];
-        }
-        __syncthreads();
-        if (t < 5) {
-          unsigned long long s = 0;
-          for (int w = 0; w < kThreads / 32; w++) s += red[w][t];
-          atomicAdd((unsigned long long *)&A.acc[((size_t)tl.item * 16 + set) * 5 + t], s);
-        }
-      }
-    }
-    __syncthreads();
-  }
-}
-
-// Rust's saturating `f64 as i32` (NaN -> 0)
-__device__ __forceinline__ int sat_i32(double v) {
-  return v != v ? 0 : v >= 2147483647.0 ? INT_MAX : v <= -2147483648.0 ? INT_MIN : (int)v;
-}
-
-// sgrproj_solve's closing arithmetic (lrf.rs:1051-1095).  The sums are exact integers: |s|, |f1 - u|,
-// |f2 - u| < 2^17, so a product is below 2^34 and a 256x256 unit's total below 2^50 < 2^53; the
-// reference's f64 accumulation of i64 line sums therefore equals the i64 total converted once.  The
-// explicit _rn intrinsics keep nvcc from contracting or reordering the reference's f64 operations.
-__global__ void lrf_search_solve(const __grid_constant__ SearchArgs A) {
-  for (uint32_t k = blockIdx.x * blockDim.x + threadIdx.x; k < A.n_items * (uint32_t)A.nsets;
-       k += gridDim.x * blockDim.x) {
-    const uint32_t item = k / A.nsets;
-    if (A.active && !A.active[A.items[item].area]) continue;
-    const int set = set_of(A, (int)(k % A.nsets));
-    const Geo g = A.geo[item];
-    const long long *acc = &A.acc[((size_t)item * 16 + set) * 5];
-    const double n = __dmul_rn((double)g.vis_w, (double)g.vis_h);
-    const double h00 = __ddiv_rn((double)acc[0], n), h11 = __ddiv_rn((double)acc[1], n);
-    const double h01 = __ddiv_rn((double)acc[2], n), h10 = h01;
-    const double sc = __ddiv_rn(128.0, n);
-    const double c0 = __dmul_rn((double)acc[3], sc), c1 = __dmul_rn((double)acc[4], sc);
-    int xq0 = 0, xq1 = 0;
-    if (kSgrS[set][0] == 0) {
-      if (h11 != 0.) xq1 = sat_i32(round(__ddiv_rn(c1, h11)));
-    } else if (kSgrS[set][1] == 0) {
-      if (h00 != 0.) xq0 = sat_i32(round(__ddiv_rn(c0, h00)));
-    } else {
-      const double det = __fma_rn(h00, h11, -__dmul_rn(h01, h10));
-      if (det != 0.) {
-        const double div1 = __fma_rn(h11, c0, -__dmul_rn(h01, c1));
-        const double div2 = __fma_rn(h00, c1, -__dmul_rn(h10, c0));
-        xq0 = sat_i32(round(__ddiv_rn(div1, det)));
-        xq1 = sat_i32(round(__ddiv_rn(div2, det)));
-      }
-    }
-    const int xqd0 = min(max(xq0, -96), 31);
-    // (1 << SGRPROJ_PRJ_BITS) - xqd0 - xq1 in i32, wrapping as a release build computes it
-    const int xqd1 = min(max((int)(128u - (uint32_t)xqd0 - (uint32_t)xq1), -32), 95);
-    int8_t *q = &A.xq[((size_t)item * 16 + set) * 2];
-    q[0] = (int8_t)xqd0;
-    q[1] = (int8_t)xqd1;
-    if (A.out_xqd) {
-      A.out_xqd[((size_t)item * 16 + set) * 2] = (int8_t)xqd0;
-      A.out_xqd[((size_t)item * 16 + set) * 2 + 1] = (int8_t)xqd1;
-    }
-  }
+// the 32x32 tiles of item `item`'s unit, over its 8x8 blocks inside the area
+inline void lrf_item_tiles(const Geo &g, uint32_t item, std::vector<Tile> &tiles) {
+  for (int ty = 0; ty < g.eh; ty += kT)
+    for (int tx = 0; tx < g.ew; tx += kT) tiles.push_back(Tile{item, (uint16_t)tx, (uint16_t)ty});
 }
 
 // count_quniform / count_subexp / recenter / count_signed_subexp_with_ref (ec.rs:381-389, 639-773)
@@ -393,64 +251,6 @@ __device__ uint32_t lrf_rate(const Rec &it, int type, int set, int x0, int x1) {
   if (kSgrS[set][0]) bits += count_signed_subexp_with_ref(x0, -96, 32, 4, it.sgrproj_ref[0]);
   if (kSgrS[set][1]) bits += count_signed_subexp_with_ref(x1, -32, 96, 4, it.sgrproj_ref[1]);
   return bits;
-}
-
-__global__ void lrf_search_decide(const __grid_constant__ SearchArgs A) {
-  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < A.n_items; i += gridDim.x * blockDim.x) {
-    b200_lrf_search_item it = A.items[i];
-    if (A.active && !A.active[it.area]) continue;
-    if (A.inc) {  // the incumbent carried from the previous restoration stage
-      it.incoming = A.inc[A.unit_of[i]];
-      it.incoming_cost = A.inc_cost[A.unit_of[i]];
-    }
-    const uint32_t ds = A.dist_scale[A.geo[i].p];
-    b200_lrf_unit best = it.incoming;
-    double best_cost = it.incoming_cost;
-    {  // None, rated with the incoming filter (rdo.rs:2633-2638)
-      const unsigned long long e = ((unsigned long long)ds * A.err[(size_t)i * kCands] + (1u << 13)) >> 14;
-      const double c = rd_cost(A.lambda, lrf_rate(it, it.incoming.type, it.incoming.set, it.incoming.xqd[0],
-                                                  it.incoming.xqd[1]), e);
-      if (A.out_err) A.out_err[(size_t)i * kCands] = e;
-      if (A.out_cand_cost) A.out_cand_cost[(size_t)i * kCands] = c;
-      if (best_cost < 0. || c < best_cost) {
-        best_cost = c;
-        best = b200_lrf_unit{};
-      }
-    }
-    for (int si = 0; si < A.nsets; si++) {
-      const int set = set_of(A, si);
-      const int8_t *q = &A.xq[((size_t)i * 16 + set) * 2];
-      const size_t slot = (size_t)i * kCands + 1 + set;
-      const unsigned long long e = ((unsigned long long)ds * A.err[slot] + (1u << 13)) >> 14;
-      const double c = rd_cost(A.lambda, lrf_rate(it, 2, set, q[0], q[1]), e);
-      if (A.out_err) A.out_err[slot] = e;
-      if (A.out_cand_cost) A.out_cand_cost[slot] = c;
-      if (c < best_cost) {
-        best_cost = c;
-        best = b200_lrf_unit{};
-        best.type = 2;
-        best.set = (uint8_t)set;
-        best.xqd[0] = q[0];
-        best.xqd[1] = q[1];
-      }
-    }
-    A.best[i] = best;
-    A.cost[i] = best_cost;
-    // RestorationFilter::notequal (lrf.rs:139-160)
-    const bool ne = it.incoming.type != best.type ||
-                    (best.type == 2 && !(it.incoming.set == best.set && it.incoming.xqd[0] == best.xqd[0] &&
-                                         it.incoming.xqd[1] == best.xqd[1]));
-    A.changed[i] = ne;
-    if (A.inc) {  // rdo.rs:2730-2741
-      const uint32_t u = A.unit_of[i];
-      A.inc_cost[u] = best_cost;
-      if (ne) {
-        A.inc[u] = best;
-        A.written[u] = 1;
-        A.area_changed[it.area] = 1;
-      }
-    }
-  }
 }
 
 }  // namespace
