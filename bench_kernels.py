@@ -963,6 +963,195 @@ def tx_size_type(ctx):
              extra={"candidates_evaluated": evaluated, "same_as_oracle": same, "library": lib})
 
 
+def host_gather(stats, prev, wib, hib, tile, x4, y4, w, h):
+    """get_subset_predictors (me.rs:386-534, CORNER, ssdec 0) for a batch of blocks of one size and slot, vectorised:
+    -> (CAND_DTYPE list grouped by block, CSR offsets), all_mvs order"""
+    x4, y4 = x4.astype(np.int64), y4.astype(np.int64)
+    x_min = np.maximum(-x4 * 32 - (128 + 8 * w), -(1 << 14) + 1)
+    x_max = np.minimum((wib - x4 - w // 4) * 32 + 128 + 8 * w, (1 << 14) - 1)
+    y_min = np.maximum(-y4 * 32 - (128 + 8 * h), -(1 << 14) + 1)
+    y_max = np.minimum((hib - y4 - h // 4) * 32 + 128 + 8 * h, (1 << 14) - 1)
+    tx, ty = x4 // tile * tile, y4 // tile * tile
+    cols, rows = np.minimum(tile, wib - tx), np.minimum(tile, hib - ty)
+    bx, by = x4 - tx, y4 - ty
+    wb, hb = w // 4, h // 4
+    chw, chh = np.minimum(wb >> 1, cols - 1 - bx), np.minimum(hb >> 1, rows - 1 - by)
+
+    def proc(g, x, y):
+        s = g[np.clip(y, 0, hib - 1), np.clip(x, 0, wib - 1)]
+        q = lambda v: np.fix(v.astype(np.int64) / 8).astype(np.int64) * 8  # noqa: E731  (i16 `/ 8`, toward zero)
+        return np.clip(q(s["mv_row"]), y_min, y_max), np.clip(q(s["mv_col"]), x_min, x_max)
+    one = np.ones(len(x4), bool)
+    cols_ = [(proc(stats, tx + bx + chw, ty + by + chh), one),
+             (proc(stats, tx + bx - 1, ty + by + chh), bx > 0),
+             (proc(stats, tx + bx + chw, ty + by - 1), by > 0),
+             (proc(stats, tx + bx + wb, ty + by + chh), bx + wb < cols),
+             (proc(stats, tx + bx + chw, ty + by + hb), by + hb < rows),
+             ((0 * x4, 0 * x4), one)]
+    if prev is not None:
+        hw, hh = np.minimum(wb >> 1, wib - 1 - x4), np.minimum(hb >> 1, hib - 1 - y4)
+        cols_ += [(proc(prev, x4 - 1, y4 + hh), x4 > 0), (proc(prev, x4 + hw, y4 - 1), y4 > 0),
+                  (proc(prev, x4 + wb, y4 + hh), x4 + wb < wib), (proc(prev, x4 + hw, y4 + hb), y4 + hb < hib),
+                  (proc(prev, x4 + hw, y4 + hh), one)]
+    rows_m = np.stack([c[0][0] for c in cols_], 1)
+    cols_m = np.stack([c[0][1] for c in cols_], 1)
+    keep = np.stack([c[1] for c in cols_], 1)
+    offs = np.zeros(len(x4) + 1, np.uint32)
+    offs[1:] = np.cumsum(keep.sum(1))
+    preds = np.zeros(int(offs[-1]), B.CAND_DTYPE)
+    preds["mv_row"], preds["mv_col"] = rows_m[keep], cols_m[keep]
+    preds["block"] = np.nonzero(keep)[0]
+    return preds, offs
+
+
+def encode_me(ctx):
+    """b200_estimate_motion_dev on a 1080p 8-bit frame x 3 reference slots: every 8x8, 16x16 and 32x32 block, and a
+    mixed partition (each 32x32 cell split into one of 32x32 .. 8x8), with use_satd_subpel, 1/8 pel and the stats grids
+    of b200_lookahead_motion_dev (LAST's grids as subset C).  Next to it, the same results through the composed
+    host-orchestrated chain (grids downloaded, predictors gathered on the host, b200_me_search_multi_dev,
+    b200_me_candidates_multi_dev with SATD, b200_subpel_search_dev per slot), compared in the same run, and the oracle
+    (oracle/encode_me.c) on 8 threads."""
+    import time
+    from tests.test_lookahead_me_gpu import dev_pyramid
+    from tests.test_oracle_encode_me import ITEM_DTYPE, TX_SIZES, Enc, grid_dims
+    lib = os.path.basename(B.LIB_PATH)
+    W, H, PAD, NS = 1920, 1080, 96, 3
+    e = Enc(W, H, bd=8, nslots=NS, tiles=(64, 64), prev=False, seed=31, pad=PAD, use_satd=1, allow_hp=1,
+            me_lambda=3.0)
+    wib, hib = grid_dims(W, H)
+    dcur, dold = dev_pyramid(e.src_img), dev_pyramid(np.ascontiguousarray(np.roll(e.src_img, 3, 1)))
+    drefs = [dev_pyramid(r) for r in e.ref_imgs]
+    d_stats, d_prev = dev(np.zeros(NS * wib * hib * 8, np.uint8)), dev(np.zeros(NS * wib * hib * 8, np.uint8))
+    lp = B.LookaheadMeParams(8, 0, e.me_lambda, 0, 1, 64, 64)
+    ctx.lookahead_motion_dev([dold] * NS, drefs, lp, d_prev)
+    ctx.lookahead_motion_dev([dcur] * NS, drefs, lp, d_stats)
+    torch.cuda.synchronize()
+    e.stats = d_stats.cpu().numpy().view(ME_STATS).reshape(NS, hib, wib)
+    e.prev = d_prev.cpu().numpy().view(ME_STATS).reshape(NS, hib, wib)
+    e.has_prev = [1] * NS
+    src = ctx.plane_from_host(e.src_img, PAD)
+    refs = [ctx.plane_from_host(r, PAD) for r in e.ref_imgs]
+    pairs = B.PlanePairs([src] * NS, refs, [0] * NS, [0] * NS)
+    rng = np.random.default_rng(5)
+
+    def grid_of(s):
+        bw, bh = TX_SIZES[s]
+        xs, ys = np.meshgrid(np.arange(0, W // 4 - bw // 4 + 1, bw // 4), np.arange(0, H // 4 - bh // 4 + 1, bh // 4))
+        return xs.ravel(), ys.ravel()
+    splits = [3, 10, 9, 2, 8, 7, 1]   # 32x32, 32x16, 16x32, 16x16, 16x8, 8x16, 8x8 (TxSize)
+    mixed = {s: ([], []) for s in splits}
+    for y in range(0, H - 31, 32):
+        for x in range(0, W - 31, 32):
+            s = splits[int(rng.integers(0, len(splits)))]
+            bw, bh = TX_SIZES[s]
+            for yy in range(y, y + 32, bh):
+                for xx in range(x, x + 32, bw):
+                    mixed[s][0].append(xx // 4)
+                    mixed[s][1].append(yy // 4)
+    loads = [(f"{TX_SIZES[s][0]}x{TX_SIZES[s][1]}", {s: grid_of(s)}) for s in (1, 2, 3)]
+    loads.append(("mixed 32x32 .. 8x8 partition", {s: (np.array(v[0]), np.array(v[1])) for s, v in mixed.items()}))
+    p_enc = B.EncMeParams(8, 1, e.me_lambda, 1, 0, 64, 64)
+    lam = e.lam()
+    for label, groups in loads:
+        parts, size_end = [], np.zeros(19, np.uint32)
+        for s in range(19):
+            if s in groups:
+                xs, ys = groups[s]
+                it = np.zeros(NS * len(xs), ITEM_DTYPE)
+                it["x4"], it["y4"] = np.tile(xs, NS), np.tile(ys, NS)
+                it["slot"] = np.repeat(np.arange(NS), len(xs))
+                it["pmv"] = rng.integers(-4, 5, (len(it), 2, 2)) * 8
+                parts.append(it)
+            size_end[s] = sum(len(p) for p in parts)
+        items = np.ascontiguousarray(np.concatenate(parts))
+        n = len(items)
+        d_items, d_out = dev(items), torch.empty(16 * n, dtype=torch.uint8, device="cuda")
+        l0 = ctx.launches
+        ctx.estimate_motion_dev(src, refs, d_stats, p_enc, size_end, d_items, n, d_out, d_prev, e.has_prev)
+        nlaunch = ctx.launches - l0
+        ms = timed(lambda: ctx.estimate_motion_dev(src, refs, d_stats, p_enc, size_end, d_items, n, d_out, d_prev,
+                                                   e.has_prev), reps=10)
+        got = d_out.cpu().numpy().view(B.ME_RESULT_DTYPE).copy()
+
+        def composed():
+            st = d_stats.cpu().numpy().view(ME_STATS).reshape(NS, hib, wib)
+            pv = d_prev.cpu().numpy().view(ME_STATS).reshape(NS, hib, wib)
+            out = np.zeros(n, B.ME_RESULT_DTYPE)
+            lo = 0
+            for s in range(19):
+                hi = int(size_end[s])
+                if hi == lo:
+                    continue
+                w, h = TX_SIZES[s]
+                it = items[lo:hi]
+                m = hi - lo
+                lists, ends = [], []
+                for k in range(NS):
+                    sel = it["slot"] == k
+                    pr, of = host_gather(st[k], pv[k], wib, hib, 16 * 64, it["x4"][sel], it["y4"][sel], w, h)
+                    lists.append((pr, of))
+                    ends.append(int(sel.sum()))
+                base = np.concatenate([[0], np.cumsum(ends)])
+                preds = np.concatenate([pr for pr, _ in lists])
+                coff = np.concatenate([[0], np.cumsum([len(pr) for pr, _ in lists])])
+                offs = np.concatenate([[0]] + [of[1:] + coff[k] for k, (_, of) in enumerate(lists)]).astype(np.uint32)
+                blocks = np.zeros(m, B.BLOCK_DTYPE)
+                blocks["x"], blocks["y"] = it["x4"] * 4, it["y4"] * 4
+                pmv = np.ascontiguousarray(it["pmv"].astype(np.int16))
+                d_b, d_pm = dev(blocks), dev(pmv)
+                pp = B.PlanePairs([src] * NS, refs, base[1:], base[1:])
+                p_sad = B.me_params(w, h, W, H, lam, allow_hp=True)
+                p_satd = B.me_params(w, h, W, H, lam, allow_hp=True, use_satd=True)
+                d_best = torch.empty(16 * m, dtype=torch.uint8, device="cuda")
+                ctx.me_search_multi_dev(pp, d_b, m, dev(preds), dev(offs), 1, p_sad, d_best, d_pm)
+                full = d_best.cpu().numpy().view(B.ME_RESULT_DTYPE).copy()
+                c = np.zeros(m, B.CAND_DTYPE)
+                c["block"] = np.arange(m)
+                c["mv_row"], c["mv_col"] = full["mv_row"], full["mv_col"]
+                d_sad, d_cost = torch.empty(4 * m, dtype=torch.uint8, device="cuda"), torch.empty(8 * m, dtype=torch.uint8,
+                                                                                                device="cuda")
+                ctx.me_candidates_multi_dev(pp, d_b, m, dev(c), m, p_satd, None, d_pm, d_sad, d_cost)
+                full["sad"] = d_sad.cpu().numpy().view(np.uint32)
+                full["cost"] = d_cost.cpu().numpy().view(np.uint64)
+                d_full, d_res = dev(full), torch.empty(16 * m, dtype=torch.uint8, device="cuda")
+                for k in range(NS):
+                    a, b = int(base[k]), int(base[k + 1])
+                    ctx.subpel_search_dev(src, refs[k], d_b[4 * a:4 * b], b - a, d_full[16 * a:16 * b], p_satd,
+                                          d_res[16 * a:16 * b], 0, d_pmv=d_pm[8 * a:8 * b])
+                out[lo:hi] = d_res.cpu().numpy().view(B.ME_RESULT_DTYPE)
+                lo = hi
+            return out
+        want = composed()
+        same = bool(got.tobytes() == want.tobytes())
+        assert same, f"encode ME {label}: the composed chain and b200_estimate_motion_dev disagree"
+        reps, t0 = 0, time.perf_counter()
+        while reps < 2 or time.perf_counter() - t0 < 1.0:
+            composed()
+            reps += 1
+        host_ms = (time.perf_counter() - t0) * 1e3 / reps
+        oracle = e.oracle(items, size_end, threads=8)
+        same_oracle = bool(oracle.tobytes() == got.tobytes())
+        assert same_oracle, f"encode ME {label}: the oracle and b200_estimate_motion_dev disagree"
+        cpu = cpu_rate(lambda: e.oracle(items, size_end, threads=8), n)
+        moved = int((((got["mv_row"] | got["mv_col"]) & 7) != 0).sum())
+        emit(f"estimate_motion_dev 1080p 8-bit x {NS} slots, {label}", n, "items", ms, 0,
+             "items = (block, slot); one call, one launch per size group; data-dependent work per item (no byte figure)",
+             cpu=cpu, cpu_threads=8,
+             extra={"launches": nlaunch, "composed_chain_ms": host_ms, "composed_over_call": host_ms / ms,
+                    "composed_chain": "grids to host, numpy gather, me_search_multi + me_candidates_multi (SATD) + "
+                                      "subpel_search per slot, per size group; host clock",
+                    "same_as_composed_chain": same, "same_as_oracle": same_oracle, "subpel_vectors": moved,
+                    "library": lib})
+    for pyr in [dcur, dold] + drefs:
+        for q in pyr:
+            ctx.plane_free(q)
+    for q in [src] + refs:
+        ctx.plane_free(q)
+
+
+ME_STATS = np.dtype([("mv_row", "<i2"), ("mv_col", "<i2"), ("normalized_sad", "<u4")])
+
+
 def main():
     torch.cuda.set_device(0)
     stream = torch.cuda.Stream()
@@ -1004,6 +1193,9 @@ def main():
         return
     if "--tx-size-type" in sys.argv[1:]:
         tx_size_type(ctx)
+        return
+    if "--encode-me" in sys.argv[1:]:
+        encode_me(ctx)
         return
     rng = np.random.default_rng(0)
     W, H, PAD = 1920, 1080, 96

@@ -200,9 +200,11 @@ int b200_me_candidates_multi_dev(b200_ctx *ctx, size_t npairs, const b200_plane 
  *               d_thresh[nblocks] = the caller's `thresh` (:771-772), umh_range = 24 (:806) or 0
  *               to stop before the UMH stage.
  * d_subset_offsets: nblocks * nsubsets + 1 offsets into d_preds (b200_cand.block is ignored).
- * Predictor gathering (get_subset_predictors, :381-533) stays with the caller: it reads the
- * neighbouring blocks' results of the same pass.  A block whose candidates are all out of range
- * (where the reference would assert) yields the empty result. */
+ * Predictor gathering (get_subset_predictors, :381-533) stays with the caller of this call.  For
+ * encode-time motion search (estimate_motion with a pmv) use b200_estimate_motion_dev, which gathers the
+ * predictors from the lookahead's stats grids on the device and adds the SATD re-measure and the sub-pel
+ * stage.  A block whose candidates are all out of range (where the reference would assert) yields the
+ * empty result. */
 int b200_me_search_dev(b200_ctx *ctx, const b200_plane *cur, const b200_plane *ref,
                        const b200_block *d_blocks, size_t nblocks, const b200_cand *d_preds,
                        const uint32_t *d_subset_offsets, int nsubsets, const int16_t *d_pmv,
@@ -523,6 +525,63 @@ typedef struct {
 int b200_lookahead_motion_dev(b200_ctx *ctx, size_t npairs, const b200_plane *curs, const b200_plane *refs,
                               const b200_lookahead_me_params *p, const b200_me_stats *d_prev,
                               const uint8_t *has_prev, b200_me_stats *d_stats);
+
+/* ---------------------------------------------------------------- encode-time motion search (me.rs:536-632)
+ * estimate_motion(fi, ts, w, h, tile_bo, ref, Some(pmv), CORNER { right: true, bottom: true }, false, 0, None) as
+ * inter_frame_rdo_mode_decision calls it (rdo.rs:1164-1196), for a batch of (block, reference slot) items of any
+ * of the 19 block sizes 4x4 .. 64x64, in one call:
+ *   - get_mv_range (me.rs:339-362) of the w x h block at frame 4x4 offset (x4, y4);
+ *   - get_subset_predictors (me.rs:386-534) in CORNER mode: left, top, right and bottom neighbours and the centre
+ *     from d_stats[slot] in the block's tile (tile-local offsets; the uniform grid of tile_w_sb x tile_h_sb
+ *     superblocks over the 8-aligned frame, the last tiles cropped; right / bottom only inside the tile), the zero
+ *     vector, and subset C from d_prev[slot] in frame coordinates when has_prev[slot]; each through process_cand
+ *     (quantize_to_fullpel, then clamp to the range);
+ *   - full_pixel_me's non-extensive branch over all_mvs() (get_best_predictor + fullpel_diamond_search);
+ *   - with use_satd_subpel, best.rd = get_fullpel_mv_rd with SATD at best.mv (me.rs:596-616);
+ *   - sub_pixel_me (me.rs:857-882): subpel_diamond_search with fi.default_filter = filter_mode, to 1/8 pel with
+ *     allow_high_precision_mv, SATD or SAD by use_satd_subpel.
+ * lambda = (me_lambda * 256.0 * 0.5) as u32 (me.rs:549-552).  d_out[i] = the MotionSearchResult of item i.
+ *
+ * Every input is final before the encode pass: both stats grids are filled by compute_motion_vectors and the
+ * encode pass never writes them, so once a block's mv stack (find_mvrefs) is known its items are independent.
+ * Which blocks share a call is the caller's business.
+ *
+ * src: the full-resolution source luma; refs: HOST array of nslots (1..7) reconstructed luma planes (fi.rec_buffer
+ * slots, indexed by ref_frame.to_index()), all of src's size and bpp.  d_stats: nslots grids of this frame in
+ * b200_lookahead_motion_dev's layout (its output passed unchanged); d_prev: NULL, or nslots grids of LAST's stats;
+ * has_prev: HOST flags per slot, required with d_prev and only with it.  Items are grouped by block size in TxSize
+ * order (4x4, 8x8, 16x16, 32x32, 64x64, 4x8, 8x4, 8x16, 16x8, 16x32, 32x16, 32x64, 64x32, 4x16, 16x4, 8x32, 32x8,
+ * 16x64, 64x16): size s owns items [size_end[s-1], size_end[s]) (HOST array; size_end[18] = nitems).  One launch per
+ * non-empty size group; no host synchronisation.
+ *
+ * Rejected with B200_ERR_ARG before anything is enqueued: nslots outside 1..7; mixed bpp or plane sizes; bit_depth
+ * not 8 for bpp 1 or not 10 / 12 for bpp 2; a row pitch that is not a multiple of 4 bytes; a tile size of 0;
+ * filter_mode outside 0..3; d_prev without has_prev or has_prev without d_prev; size_end decreasing or not ending
+ * at nitems; and a pad on any plane below what the mv range plus the 8-tap footprint (-3 .. +4) needs.  With W8 /
+ * H8 = width / height rounded up to 8, every plane's pad must be at least
+ *   max(w + 19, W8 - width + w + 20, h + 19, H8 - height + h + 20)
+ * for the largest w and h of the non-empty size groups (e.g. 84 for 64x64 blocks of a 1920x1080 frame).  Above that
+ * pad no footprint reaches past the readable border, so PlaneSlice::clamp (predict.rs:296) never moves one.
+ * An item whose slot is >= nslots or whose (x4, y4) lies outside the frame's 4x4 grid (2 * ceil(width / 8) x
+ * 2 * ceil(height / 8)) gets the empty result {UINT64_MAX, UINT32_MAX, 0, 0} and reads nothing; so does an item whose
+ * candidates are all out of range (never the case for a valid item: the zero vector is always in range). */
+typedef struct {
+  uint16_t x4, y4;   /* frame block offset in 4x4 units (PlaneBlockOffset) */
+  uint8_t slot;      /* reference slot index, 0 .. nslots-1 (ref_frame.to_index()) */
+  uint8_t pad_;
+  int16_t pmv[2][2]; /* (row, col) of mv_stack[0].this_mv, mv_stack[1].this_mv, 1/8 pel (rdo.rs:1174-1180) */
+} b200_enc_me_item;  /* 14 B */
+typedef struct {
+  int32_t bit_depth, allow_high_precision_mv;
+  double me_lambda;         /* fi.me_lambda */
+  int32_t use_satd_subpel;  /* speed_settings.motion.use_satd_subpel */
+  int32_t filter_mode;      /* fi.default_filter, as b200_subpel_search_dev takes it */
+  int32_t tile_w_sb, tile_h_sb;
+} b200_enc_me_params;
+int b200_estimate_motion_dev(b200_ctx *ctx, const b200_plane *src, size_t nslots, const b200_plane *refs,
+                             const b200_me_stats *d_stats, const b200_me_stats *d_prev, const uint8_t *has_prev,
+                             const b200_enc_me_params *p, const uint32_t size_end[19],
+                             const b200_enc_me_item *d_items, size_t nitems, b200_me_result *d_out);
 
 /* ---------------------------------------------------------------- temporal RDO (api/internal.rs, rdo.rs)
  * compute_block_importances (internal.rs:1075-1230): the mbtree-style propagation of block importances

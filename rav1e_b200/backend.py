@@ -73,6 +73,18 @@ class LookaheadMeParams(C.Structure):
 ME_STATS_DTYPE = np.dtype([("mv_row", "<i2"), ("mv_col", "<i2"), ("normalized_sad", "<u4")])
 
 
+class EncMeParams(C.Structure):
+    """b200_enc_me_params: the frame's settings for b200_estimate_motion_dev."""
+    _fields_ = [("bit_depth", C.c_int32), ("allow_high_precision_mv", C.c_int32), ("me_lambda", C.c_double),
+                ("use_satd_subpel", C.c_int32), ("filter_mode", C.c_int32), ("tile_w_sb", C.c_int32),
+                ("tile_h_sb", C.c_int32)]
+
+
+# b200_enc_me_item: frame 4x4 offset, reference slot, the two mv-stack predictors (row, col)
+ENC_ME_ITEM_DTYPE = np.dtype([("x4", "<u2"), ("y4", "<u2"), ("slot", "u1"), ("pad_", "u1"), ("pmv", "<i2", (2, 2))])
+assert ENC_ME_ITEM_DTYPE.itemsize == 14
+
+
 def imp_steps(steps):
     """[(src, dst, len, mv_index), ...] -> a ctypes array of ImpStep (execution order)."""
     arr = (ImpStep * max(len(steps), 1))()
@@ -303,6 +315,7 @@ def lib():
     L.b200_intra_tx_size_type_dev.argtypes = [vp, pp, pp] + [i32] * 9 + [C.c_double, C.c_uint32, vp, sz, vp, sz,
                                                                           vp, sz, vp, vp]
     L.b200_lookahead_motion_dev.argtypes = [vp, sz, vp, vp, C.POINTER(LookaheadMeParams), vp, vp, vp]
+    L.b200_estimate_motion_dev.argtypes = [vp, pp, sz, vp, vp, vp, vp, C.POINTER(EncMeParams), vp, vp, sz, vp]
     L.b200_get_intra_edges_dev.argtypes = [vp, pp] + [i32] * 7 + [vp, sz, vp, vp]
     L.b200_pred_cfl_ac_dev.argtypes = [vp, pp, vp, sz] + [i32] * 6 + [vp]
     L.b200_intra_mode_screen_dev.argtypes = [vp, pp, pp] + [i32] * 6 + [vp, sz, vp, vp]
@@ -493,6 +506,23 @@ class Context:
         self.check(self.L.b200_lookahead_motion_dev(self.h, n, C.addressof(arrs[0]), C.addressof(arrs[1]),
                                                     C.byref(params), _dev_ptr(d_prev), _np_ptr(flags),
                                                     _dev_ptr(d_stats)))
+
+    def estimate_motion_dev(self, src, refs, d_stats, params, size_end, d_items, nitems, d_out, d_prev=None,
+                            has_prev=None):
+        """estimate_motion for a batch of (block, reference slot) items (include/b200rdo.h): src a Plane, refs a
+        list of Plane (one per slot); d_stats / d_prev len(refs) ME_STATS_DTYPE grids on the device; size_end the
+        19 cumulative item counts in TxSize order; d_items ENC_ME_ITEM_DTYPE, d_out ME_RESULT_DTYPE."""
+        n = len(refs)
+        arr = (Plane * max(n, 1))()
+        for k, p in enumerate(refs):
+            C.memmove(C.byref(arr[k]), C.byref(p), C.sizeof(Plane))
+        ends = np.ascontiguousarray(np.asarray(size_end, np.uint32).reshape(19))
+        flags = None
+        if has_prev is not None:
+            flags = np.ascontiguousarray(np.asarray(has_prev, np.uint8).reshape(n))
+        self.check(self.L.b200_estimate_motion_dev(self.h, C.byref(src), n, C.addressof(arr), _dev_ptr(d_stats),
+                                                   _dev_ptr(d_prev), _np_ptr(flags), C.byref(params),
+                                                   ends.ctypes.data, _dev_ptr(d_items), nitems, _dev_ptr(d_out)))
 
     # ---- temporal RDO
     def block_importances_dev(self, frames, bit_depth, d_intra_costs, d_mvs, steps, d_importances):

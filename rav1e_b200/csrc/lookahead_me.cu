@@ -170,31 +170,6 @@ __global__ void __launch_bounds__(128) refine_kernel(const __grid_constant__ LaA
   }
 }
 
-// The block's predictor subsets, gathered identically by every lane and published through shared memory.
-struct SmemPreds {
-  const short2 *list;  // (row, col)
-  const uint32_t *offs;
-  __device__ __forceinline__ void span(int s, uint32_t &lo, uint32_t &hi) const {
-    lo = offs[s];
-    hi = offs[s + 1];
-  }
-  __device__ __forceinline__ void mv(uint32_t i, int &row, int &col) const {
-    const short2 q = list[i];
-    row = q.x, col = q.y;
-  }
-};
-
-struct Gather {
-  uint32_t min_sad;
-  const BlockCtx *c;
-  __device__ __forceinline__ short2 proc(const b200_me_stats st) {  // process_cand, me.rs:405-412
-    min_sad = min(min_sad, st.normalized_sad);
-    const int col = min(max((st.mv_col / 8) * 8, c->rng.x_min), c->rng.x_max);
-    const int row = min(max((st.mv_row / 8) * 8, c->rng.y_min), c->rng.y_max);
-    return make_short2((short)row, (short)col);
-  }
-};
-
 // One anti-diagonal of one level: get_subset_predictors + full_pixel_me (+ the exhaustive grid) per block.
 template <typename T>
 __global__ void __launch_bounds__(128) diag_kernel(const __grid_constant__ LaArgs a) {
@@ -250,16 +225,8 @@ __global__ void __launch_bounds__(128) diag_kernel(const __grid_constant__ LaArg
       has_median = true;
     }
     b[nb++] = make_short2(0, 0);
-    if (a.prev && pp.has_prev) {  // subset C: LAST's final stats for this slot, frame coordinates
-      const b200_me_stats *P = a.prev + base;
-      const int W = a.w_in_b, H = a.h_in_b;
-      const int hw = min(wb >> 1, W - 1 - bx), hh = min(hb >> 1, H - 1 - by);
-      if (bx > 0) cc[nc++] = G.proc(P[(size_t)(by + hh) * W + bx - 1]);
-      if (by > 0) cc[nc++] = G.proc(P[(size_t)(by - 1) * W + bx + hw]);
-      if (bx + wb < W) cc[nc++] = G.proc(P[(size_t)(by + hh) * W + bx + wb]);
-      if (by + hb < H) cc[nc++] = G.proc(P[(size_t)(by + hb) * W + bx + hw]);
-      cc[nc++] = G.proc(P[(size_t)(by + hh) * W + bx + hw]);
-    }
+    if (a.prev && pp.has_prev)  // subset C: LAST's final stats for this slot, frame coordinates
+      nc = G.subset_c(a.prev + base, a.w_in_b, a.h_in_b, bx, by, wb, hb, cc);
     const uint32_t min_sad = (uint32_t)(((unsigned long long)G.min_sad * (unsigned long long)(w * h)) >> 14);
     auto dec = [&](short2 v) { return make_short2((short)(v.x >> s), (short)(v.y >> s)); };
     // all_mvs (one list) or median | subset_b | subset_c

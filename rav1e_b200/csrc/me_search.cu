@@ -14,9 +14,8 @@
 // almost entirely); every "if rd.cost < best.cost" chain of the reference is a first-minimum
 // argmin over the set, so the winner is found with shuffles and the data-dependent control flow
 // (move, shrink the radius, early exits) stays warp-uniform.  Predictor subsets come from the
-// caller: get_subset_predictors (me.rs:381-533) reads neighbouring blocks' results of the same
-// pass, a wavefront dependency that stays with the encoder's block order (the lookahead's own pass,
-// predictors included, is lookahead_me.cu).  The state machine itself is in me_search_dev.cuh.
+// caller here; the lookahead's own pass gathers them in lookahead_me.cu and the encode-time search
+// (estimate_motion with a pmv) in encode_me.cu.  The state machine itself is in me_search_dev.cuh.
 #include <cuda_runtime.h>
 
 #include <algorithm>

@@ -165,6 +165,46 @@ struct ListPreds {
   }
 };
 
+// Predictor subsets gathered into shared memory: offs = nsubsets + 1 offsets into list.
+struct SmemPreds {
+  const short2 *list;  // (row, col)
+  const uint32_t *offs;
+  __device__ __forceinline__ void span(int s, uint32_t &lo, uint32_t &hi) const {
+    lo = offs[s];
+    hi = offs[s + 1];
+  }
+  __device__ __forceinline__ void mv(uint32_t i, int &row, int &col) const {
+    const short2 q = list[i];
+    row = q.x, col = q.y;
+  }
+};
+
+// get_subset_predictors' steps (me.rs:386-534) shared by the lookahead (lookahead_me.cu) and the encode-time
+// search (encode_me.cu).  Every lane gathers the same values.
+struct Gather {
+  uint32_t min_sad;
+  const BlockCtx *c;
+  __device__ __forceinline__ short2 proc(const b200_me_stats st) {  // process_cand, me.rs:405-412
+    min_sad = min(min_sad, st.normalized_sad);
+    const int col = min(max((st.mv_col / 8) * 8, c->rng.x_min), c->rng.x_max);
+    const int row = min(max((st.mv_row / 8) * 8, c->rng.y_min), c->rng.y_max);
+    return make_short2((short)row, (short)col);
+  }
+  // subset C (me.rs:477-515): LAST's stats grid P (W x H cells) around the block at frame 4x4 offset (bx, by),
+  // wb x hb cells; appends left, top, right, bottom (those inside the frame) and the centre to cc
+  __device__ __forceinline__ int subset_c(const b200_me_stats *P, int W, int H, int bx, int by, int wb, int hb,
+                                          short2 *cc) {
+    int nc = 0;
+    const int hw = min(wb >> 1, W - 1 - bx), hh = min(hb >> 1, H - 1 - by);
+    if (bx > 0) cc[nc++] = proc(P[(size_t)(by + hh) * W + bx - 1]);
+    if (by > 0) cc[nc++] = proc(P[(size_t)(by - 1) * W + bx + hw]);
+    if (bx + wb < W) cc[nc++] = proc(P[(size_t)(by + hh) * W + bx + wb]);
+    if (by + hb < H) cc[nc++] = proc(P[(size_t)(by + hb) * W + bx + hw]);
+    cc[nc++] = proc(P[(size_t)(by + hh) * W + bx + hw]);
+    return nc;
+  }
+};
+
 // full_pixel_me without the exhaustive grid for the block of `c`, called by all 32 lanes (g = lane / 8,
 // sub = lane % 8); returns the same Best in every lane.  nsubsets 1: all_mvs (non-extensive); 3: median |
 // subset_b | subset_c with the `sad < thresh` exits and UMH over umh_range.  Preds: span(subset, lo, hi)

@@ -24,9 +24,7 @@
 #include <algorithm>
 
 #include "fwd_txfm_dev.cuh"
-#include "mc_dev.cuh"
-#include "me_dev.cuh"
-#include "warp_satd.cuh"
+#include "subpel_dev.cuh"
 
 namespace {
 
@@ -52,19 +50,6 @@ struct SrdoArgs {
 };
 
 template <typename T, int W, int H>
-__device__ __forceinline__ uint32_t warp_sad(const T *org, int os, const T *pred, int lane) {
-  uint32_t acc = 0;
-#pragma unroll 4
-  for (int i = lane; i < W * H; i += 32) {
-    const int r = i / W, c = i - r * W;
-    acc += (uint32_t)abs((int)org[(long long)r * os + c] - (int)pred[i]);
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-  return acc;
-}
-
-template <typename T, int W, int H>
 __global__ void __launch_bounds__(256) subpel_rdo_kernel(const __grid_constant__ SrdoArgs a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   using CoefT = typename std::conditional<sizeof(T) == 1, int16_t, int32_t>::type;
@@ -81,55 +66,21 @@ __global__ void __launch_bounds__(256) subpel_rdo_kernel(const __grid_constant__
   for (size_t blk = (size_t)blockIdx.x * nw + wid; blk < a.nblocks; blk += (size_t)gridDim.x * nw) {
     const b200_block b = a.blocks[blk];
     const uint32_t lo = a.start ? 0u : a.cand_offsets[blk], hi = a.start ? 0u : a.cand_offsets[blk + 1];
-    const MvRange rng = b200_mv_range(a.w_in_b, a.h_in_b, b.x / MI_SIZE, b.y / MI_SIZE, W, H);
-    const Pmv pm = load_pmv(a.pmv, blk);
     const T *org = (const T *)a.cur + (long long)b.y * a.cur_stride + b.x;
+    const SubpelBlock<T, W, H> sp{org, a.cur_stride, (const T *)a.ref, a.ref_stride, b.x, b.y,
+                                  b200_mv_range(a.w_in_b, a.h_in_b, b.x / MI_SIZE, b.y / MI_SIZE, W, H),
+                                  load_pmv(a.pmv, blk), a.lambda, a.allow_hp, a.use_satd, a.bit_depth, xb, yb, tile,
+                                  inter};
     T *pcur = pred0, *pbest = pred1;
     unsigned long long best_cost = kEmptyCost;
     uint32_t best_sad = kEmptySad;
     int best_row = 0, best_col = 0;
-    // get_subpel_mv_rd (me.rs:1411-1442) of one vector: prediction into `pcur`, distortion, cost
-    auto eval = [&](int mv_row, int mv_col, uint32_t &sad) -> unsigned long long {
-      sad = kEmptySad;
-      if (B200_MV_OUTSIDE(mv_row, mv_col, rng)) return kEmptyCost;
-      // predict.rs:284-297 get_mv_params (luma)
-      const int y0 = b.y + (mv_row >> 3), x0 = b.x + (mv_col >> 3);
-      const int row_frac = (int)(((unsigned)mv_row << 1) & 0xf), col_frac = (int)(((unsigned)mv_col << 1) & 0xf);
-      const T *src = (const T *)a.ref + (long long)(y0 - 3) * a.ref_stride + (x0 - 3);
-      __syncwarp();
-      mc_stage_tile<T, W, H>(tile, src, a.ref_stride, lane);
-      __syncwarp();
-      mc_put_warp<T, W, H>(tile, inter, pcur, xb, col_frac, yb, row_frac, a.bit_depth, lane);
-      __syncwarp();
-      sad = a.use_satd ? block_satd<T, W, H>(org, a.cur_stride, pcur, lane) : warp_sad<T, W, H>(org, a.cur_stride, pcur, lane);
-      return b200_mv_cost(sad, mv_row, mv_col, pm.r0, pm.c0, pm.r1, pm.c1, a.lambda, a.allow_hp);
-    };
+    auto eval = [&](int mv_row, int mv_col, uint32_t &sad) { return sp.rd(mv_row, mv_col, pcur, sad, lane); };
     if (a.start) {
-      // ---- subpel_diamond_search, me.rs:1311-1383: move to the best of the four diamond points while
-      // one is strictly better, then halve the radius (1/2 pel down to 1/4, or 1/8 with high precision)
+      // ---- subpel_diamond_search, me.rs:1311-1383 (subpel_dev.cuh)
       const b200_me_result st = a.start[blk];
       best_cost = st.cost, best_sad = st.sad, best_row = st.mv_row, best_col = st.mv_col;
-      int radius_log2 = 2;
-      const int end_log2 = a.allow_hp ? 0 : 1;
-      for (;;) {
-        unsigned long long cc = kEmptyCost;
-        uint32_t cs = kEmptySad;
-        int cr = 0, ccol = 0;
-#pragma unroll 1
-        for (int k = 0; k < 4; k++) {  // DIAMOND_R1_PATTERN_SUBPEL, me.rs:931-934: row+1, col+1, row-1, col-1
-          const int dr = (k == 0) - (k == 2), dc = (k == 1) - (k == 3);
-          const int mr = (short)(best_row + (short)(dr << radius_log2)), mc = (short)(best_col + (short)(dc << radius_log2));
-          uint32_t sad;
-          const unsigned long long cost = eval(mr, mc, sad);
-          if (cost < cc) cc = cost, cs = sad, cr = mr, ccol = mc;
-        }
-        if (best_cost <= cc) {
-          if (radius_log2 == end_log2) break;
-          radius_log2--;
-        } else {
-          best_cost = cc, best_sad = cs, best_row = cr, best_col = ccol;
-        }
-      }
+      sp.diamond(best_cost, best_sad, best_row, best_col, pcur, lane);
       if (a.tx_on && best_cost != kEmptyCost) {  // the winner's prediction for the transform below
         uint32_t sad;
         (void)eval(best_row, best_col, sad);
